@@ -226,6 +226,17 @@ LB200_EXPORT void lb200_exact_search_device(void const* d_dataset, size_t datase
                                             lb200_scalar_kind_t scalar_kind, size_t dimensions,
                                             lb200_metric_kind_t metric_kind, size_t count, lb200_key_t* d_keys,
                                             lb200_distance_t* d_distances, void* cuda_stream, lb200_error_t* error);
+/* Test hook, not a search entry point: lb200_exact_search on dense f32 rows (l2sq or cos, count <= 192) with the
+ * tensor-core filter forced on, copying the filter's intermediate buffers out; host memory.  plan[2] receives the row
+ * groups G and the candidates per list KP, eps[4] the error-bound constants (relative, summation, linear, absolute).
+ * With cand_d == NULL nothing runs: call once that way to size the buffers qn[queries_size], xn[dataset_size],
+ * cand_d / cand_i [queries_size][G][KP], dropped_lb [queries_size][G], unsafe [queries_size] (1 = not certified,
+ * answered by the SIMT kernels), keys / distances [queries_size][count] (the search's final answer). */
+LB200_EXPORT void lb200_exact_tc_probe(float const* dataset, size_t dataset_size, float const* queries, size_t queries_size,
+                                       size_t dimensions, lb200_metric_kind_t metric_kind, size_t count, uint32_t* plan,
+                                       float* eps, float* qn, float* xn, float* cand_d, uint32_t* cand_i, float* dropped_lb,
+                                       uint8_t* unsafe, lb200_key_t* keys, lb200_distance_t* distances,
+                                       lb200_error_t* error);
 /* f32 -> f16 / i8 / b1 (index_plugins.hpp:879-974); host memory; `count` vectors. */
 LB200_EXPORT void lb200_cast(lb200_scalar_kind_t from, void const* vectors, lb200_scalar_kind_t to, void* result,
                              size_t result_size, int dims, lb200_error_t* error);

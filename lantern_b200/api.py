@@ -122,6 +122,9 @@ SIGNATURES = {
                                   C.c_size_t, ERRP]),
     "lb200_exact_search_device": (None, [C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int,
                                          C.c_size_t, C.c_int, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, ERRP]),
+    "lb200_exact_tc_probe": (None, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_size_t,
+                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_void_p, ERRP]),
     "lb200_cast": (None, [C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_int, ERRP]),
     "lb200_cast_batch": (None, [C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_void_p, ERRP]),
     "lb200_quantize_pq": (None, [C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
@@ -441,6 +444,24 @@ def exact_search_device(d_dataset, n, d_stride, d_queries, nq, q_stride, k, d_ke
     _static("lb200_exact_search_device", C.c_void_p(d_dataset), n, d_stride, C.c_void_p(d_queries), nq, q_stride,
             SCALAR[quant], dims, METRIC[metric], k, C.c_void_p(d_keys), C.c_void_p(d_dists),
             C.c_void_p(stream) if stream else None)
+
+
+def exact_tc_probe(dataset, queries, k, metric="l2sq"):
+    """Test hook: exact_search with the tensor-core filter forced on, plus the filter's intermediate buffers (dict)."""
+    X = np.ascontiguousarray(dataset, dtype=np.float32)
+    Q = np.ascontiguousarray(queries, dtype=np.float32)
+    n, nq, d = len(X), len(Q), X.shape[1]
+    plan, eps = np.zeros(2, np.uint32), np.zeros(4, np.float32)
+    args = (_ptr(X), n, _ptr(Q), nq, d, METRIC[metric], k, _ptr(plan), _ptr(eps))
+    _static("lb200_exact_tc_probe", *args, *([None] * 8))
+    G, KP = int(plan[0]), int(plan[1])
+    out = dict(groups=G, KP=KP, eps_rel=float(eps[0]), eps_sum=float(eps[1]), eps_lin=float(eps[2]), eps_abs=float(eps[3]),
+               qn=np.zeros(nq, np.float32), xn=np.zeros(n, np.float32), cand_d=np.zeros((nq, G, KP), np.float32),
+               cand_i=np.zeros((nq, G, KP), np.uint32), dropped_lb=np.zeros((nq, G), np.float32),
+               unsafe=np.zeros(nq, np.uint8), keys=np.zeros((nq, k), np.uint64), dists=np.zeros((nq, k), np.float32))
+    _static("lb200_exact_tc_probe", *args, *(_ptr(out[f]) for f in ("qn", "xn", "cand_d", "cand_i", "dropped_lb", "unsafe",
+                                                                     "keys", "dists")))
+    return out
 
 
 def cast(vectors_f32, quant):

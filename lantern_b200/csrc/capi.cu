@@ -533,6 +533,35 @@ LB200_EXPORT void lb200_exact_search(void const* dataset, size_t dataset_size, s
     });
 }
 
+LB200_EXPORT void lb200_exact_tc_probe(float const* dataset, size_t dataset_size, float const* queries, size_t queries_size,
+                                       size_t dimensions, lb200_metric_kind_t metric_kind, size_t count, uint32_t* plan,
+                                       float* eps, float* qn, float* xn, float* cand_d, uint32_t* cand_i, float* dropped_lb,
+                                       uint8_t* unsafe, lb200_key_t* keys, lb200_distance_t* distances, lb200_error_t* error) {
+    guarded(error, [&] {
+        require_device();
+        check_metric_scalar(metric_kind, lb200_scalar_f32_k);
+        const int dm = distance_mode(metric_kind, SK_F32);
+        if (!plan || !eps || !queries_size || !count || (dm != DM_L2SQ && dm != DM_COS) || !dataset_size || count > 192)
+            throw CudaError("exact_tc_probe: needs plan, eps, l2sq or cos, queries, rows and 1 <= count <= 192");
+        const size_t rb = round_up(dimensions * 4, 16);
+        const ExactTcPlan pl = exact_tc_plan(dataset_size, queries_size, count, (uint32_t)rb);
+        plan[0] = pl.groups, plan[1] = pl.KP;
+        eps[0] = pl.eps.rel, eps[1] = pl.eps.sum, eps[2] = pl.eps.lin, eps[3] = pl.eps.abs;
+        if (!cand_d)
+            return;
+        if (!qn || !xn || !cand_i || !dropped_lb || !unsafe || !keys || !distances)
+            throw CudaError("exact_tc_probe: null output buffer");
+        DeviceTemp dd(dataset_size * rb), dq(queries_size * rb), dk(queries_size * count * 8), dv(queries_size * count * 4);
+        upload_rows(dataset, dataset_size, dimensions * 4, SK_F32, dimensions, dd.as<uint8_t>(), rb);
+        upload_rows(queries, queries_size, dimensions * 4, SK_F32, dimensions, dq.as<uint8_t>(), rb);
+        const ExactTcProbe probe{qn, xn, cand_d, cand_i, dropped_lb, unsafe};
+        launch_exact(dm, SK_F32, dd.as<uint8_t>(), dataset_size, rb, dq.as<uint8_t>(), queries_size, rb, (uint32_t)rb, count,
+                     dk.as<uint64_t>(), dv.as<float>(), 0, &probe);
+        LB_CUDA(cudaMemcpy(keys, dk.p, queries_size * count * 8, cudaMemcpyDeviceToHost));
+        LB_CUDA(cudaMemcpy(distances, dv.p, queries_size * count * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
 LB200_EXPORT void lb200_cast_batch(void const* vectors_f32, size_t count, size_t dims, lb200_scalar_kind_t to, void* result,
                                    lb200_error_t* error) {
     guarded(error, [&] {

@@ -147,6 +147,15 @@ __device__ __forceinline__ float cos_from_parts(float ab, float a2, float b2) {
     return 1.f - ab / (sqrtf(a2) * sqrtf(b2));
 }
 
+// Order of the exhaustive search's results: by distance, ties by lower offset; a NaN distance (a row or query holding NaN
+// or opposite infinities) ranks after every number, +inf included, as in numpy's sort.  A plain `<` would let a NaN enter
+// a sorted list anywhere and stay there.
+template <typename I> __device__ __forceinline__ bool closer_total(float d, I id, float od, I oid) {
+    if (d != d || od != od)
+        return od != od && (d == d || id < oid);
+    return d < od || (d == od && id < oid);
+}
+
 // ---- warp-reduce the partials into the final distance (all lanes receive it) ------------------------
 template <int DM, int SK> __device__ __forceinline__ float finish_distance(const DistAcc<DM, SK>& a, float a2) {
     if constexpr (DM == DM_HAMMING) {

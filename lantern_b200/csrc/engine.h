@@ -207,10 +207,30 @@ void launch_search(int dist_mode, int scalar_kind, bool pq, const SearchLaunch& 
 // group.cu: the warp-per-query kernel as a single-GPU search path
 void launch_warp_search(Index& idx, const uint8_t* qbuf, size_t qrow, size_t nq, size_t k, uint32_t L, uint64_t* d_keys, float* d_dists,
                         uint32_t* d_counts, cudaStream_t stream);
-// exact.cu
+// exact_tc.cu: launch plan of the tensor-core filter, and a test hook that copies its intermediate buffers to the host
+struct ExactTcEps { // |approximate - exact fp32 distance| <= eps(|q|^2, |x|^2): see approx_eps in exact_tc.cu
+    float rel;       // 3xTF32 dot product, relative to |q||x|
+    float sum;       // fp32 norms, final arithmetic and the exact kernel's own summation, relative to |q|^2 + |x|^2
+    float lin, abs;  // dot product with flushed subnormals: lin (|q| + |x|) + abs
+};
+struct ExactTcPlan {
+    uint32_t groups; // row groups per query tile
+    uint32_t KP;     // candidates kept per (query, row group)
+    ExactTcEps eps;
+};
+ExactTcPlan exact_tc_plan(size_t n, size_t nq, size_t k, uint32_t row_bytes);
+struct ExactTcProbe { // host buffers, sized from exact_tc_plan; filled by launch_exact_tc before it frees its scratch
+    float* qn;         // [nq] fp32 |q|^2 as the filter used them
+    float* xn;         // [n]  fp32 |x|^2
+    float* cand_d;     // [nq][groups][KP] approximate distances, heap order, +inf padded
+    uint32_t* cand_i;  // [nq][groups][KP] row offsets, 0xFFFFFFFF padded
+    float* dropped_lb; // [nq][groups] smallest lower bound of anything a list dropped
+    uint8_t* unsafe;   // [nq] 1 = not certified, answered by the SIMT kernels
+};
+// exact.cu.  `probe` (tests only) forces the tensor-core path and captures its buffers.
 void launch_exact(int dist_mode, int scalar_kind, const uint8_t* d_data, size_t n, size_t data_stride,
                   const uint8_t* d_queries, size_t nq, size_t q_stride, uint32_t row_bytes, size_t k, uint64_t* d_keys,
-                  float* d_dists, cudaStream_t stream);
+                  float* d_dists, cudaStream_t stream, const ExactTcProbe* probe = nullptr);
 void launch_pair_distance(int dist_mode, int scalar_kind, const uint8_t* d_a, size_t a_stride, const uint8_t* d_b,
                           size_t b_stride, size_t n, uint32_t row_bytes, float* d_out, cudaStream_t stream);
 void launch_merge_shards(const uint64_t* d_keys, const float* d_dists, size_t shards, size_t nq, size_t k,

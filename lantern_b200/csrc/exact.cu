@@ -25,9 +25,7 @@ constexpr int kQT = 8;      // queries per CTA == warps per CTA
 constexpr int kExWarps = 8; // 256 threads
 constexpr int kSub = 32;    // dataset rows per sub-batch (4 per warp)
 
-__device__ __forceinline__ bool closer(float d, uint64_t id, float od, uint64_t oid) {
-    return d < od || (d == od && id < oid);
-}
+__device__ __forceinline__ bool closer(float d, uint64_t id, float od, uint64_t oid) { return closer_total(d, id, od, oid); }
 
 // Sorted (ascending by (dist, id)) insert of one element into a list of capacity k, by a full warp.
 __device__ __forceinline__ void list_insert(float* ld, uint64_t* li, uint32_t& size, uint32_t k, float d, uint64_t id, int lane) {
@@ -284,24 +282,27 @@ void launch_merge_shards(const uint64_t* d_keys, const float* d_dists, size_t sh
 
 // exact_tc.cu
 bool exact_tc_applicable(int dist_mode, int scalar_kind, size_t n, size_t nq, size_t k, uint32_t row_bytes);
+bool exact_tc_defined(int dist_mode, int scalar_kind, size_t n, size_t k);
 void launch_exact_tc(int dist_mode, const uint8_t* d_data, size_t n, size_t data_stride, const uint8_t* d_queries, size_t nq,
                      size_t q_stride, uint32_t row_bytes, size_t k, uint64_t* d_keys, float* d_dists, uint8_t** d_unsafe,
-                     uint32_t** d_unsafe_count, cudaStream_t stream);
+                     uint32_t** d_unsafe_count, cudaStream_t stream, const ExactTcProbe* probe);
 
 void launch_exact(int dist_mode, int scalar_kind, const uint8_t* d_data, size_t n, size_t data_stride,
                   const uint8_t* d_queries, size_t nq, size_t q_stride, uint32_t row_bytes, size_t k, uint64_t* d_keys,
-                  float* d_dists, cudaStream_t stream) {
+                  float* d_dists, cudaStream_t stream, const ExactTcProbe* probe) {
     if (!nq || !k)
         return;
     if (k > 1024)
         throw CudaError("exact search: count > 1024 is not supported");
+    if (probe && !exact_tc_defined(dist_mode, scalar_kind, n, k))
+        throw CudaError("exact search probe: the tensor-core filter takes f32 l2sq / cos, 1 <= n < 2^32 rows and count <= 192");
     // f32 l2sq / cos on a GEMM-sized problem: tensor-core filter + exact re-rank (exact_tc.cu); the SIMT kernels below then
     // run only for the queries the filter could not certify (usually none: every CTA of the second pass exits at once)
     uint8_t* qmask = nullptr;
     uint32_t* unsafe_count = nullptr;
-    if (exact_tc_applicable(dist_mode, scalar_kind, n, nq, k, row_bytes))
+    if (probe || exact_tc_applicable(dist_mode, scalar_kind, n, nq, k, row_bytes))
         launch_exact_tc(dist_mode, d_data, n, data_stride, d_queries, nq, q_stride, row_bytes, k, d_keys, d_dists, &qmask, &unsafe_count,
-                        stream);
+                        stream, probe);
     size_t rows_per_block = 4096;
     if ((n + rows_per_block - 1) / rows_per_block > 1024)
         rows_per_block = round_up((n + 1023) / 1024, kSub);

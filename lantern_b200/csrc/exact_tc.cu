@@ -12,9 +12,11 @@
 //   3. exact_tc_rerank_kernel  per query: candidates whose lower bound (approx - eps) does not exceed the k-th smallest
 //                              upper bound (approx + eps) are re-measured with the SIMT distance code of exact.cu
 //                              (same lane layout, same reduction) and sorted by (distance, offset): ids and distances are
-//                              those of exact_block_kernel, ties included.  eps = (dims + 32) * 2^-24 * |q||x| covers the
-//                              split's truncation and worst-case fp32 accumulation on both sides.  A query whose lists
-//                              may have dropped a qualifying row, or with more qualifying rows than fit, is flagged and
+//                              those of exact_block_kernel, ties included.  eps (approx_eps) bounds |approx - exact fp32|:
+//                              the split's truncation and the tensor-core accumulation, the fp32 norms and the exact
+//                              kernel's own summation (both growing with the chunks per lane), and subnormal products the
+//                              tensor cores may flush.  A query whose lists may have dropped a qualifying row, with more
+//                              qualifying rows than fit, or with a non-finite approximate distance, is flagged and
 //                              answered by the SIMT kernels (exact.cu) -- never silently wrong.
 //
 // Filter kernel anatomy (one CTA per SM, 4 warpgroups, persistent over its row tiles):
@@ -29,6 +31,8 @@
 // Two shared-memory stages (64 KB each: A hi/lo 2 x 16 KB, B hi/lo 2 x 16 KB) and the 66 KB accumulator tile keep the
 // loads of k-block kb+1 under the MMAs of k-block kb, and the epilogue of tile t under the MMAs of tile t+1.
 #include <cuda_runtime.h>
+#include <float.h>
+#include <math.h>
 #include <stdlib.h>
 
 #include <type_traits>
@@ -133,7 +137,7 @@ struct TcParams {
     uint32_t groups;  // row groups per query tile: CTA (qt, g) handles row tiles g, g + groups, ...
     uint32_t row_tiles;
     uint32_t KP;
-    float eps_rel;
+    ExactTcEps eps;
     float* cand_d;    // [nq][groups][KP] approx distances of the kept rows, heap order (+inf padded)
     uint32_t* cand_i; // [nq][groups][KP]
     float* dropped_lb; // [nq][groups] smallest lower bound among entries the list could not keep (+inf if none)
@@ -150,11 +154,21 @@ template <int DM> __device__ __forceinline__ float approx_distance(float dot, fl
         return qn + xn - 2.f * dot;
     }
 }
-template <int DM> __device__ __forceinline__ float approx_eps(float eps_rel, float qn, float xn) {
-    if constexpr (DM == DM_COS)
-        return eps_rel + 3e-6f; // |dot error| / (|q||x|), plus norms, square roots and the division in fp32
-    else
-        return 2.f * eps_rel * sqrtf(qn) * sqrtf(xn) + 2e-6f * (qn + xn); // dot error; norms and the final sum in fp32
+// Bound on |approx_distance - the exact kernel's fp32 distance| (derivation in exact_tc_plan).  +inf where no bound holds:
+// cos with a norm that is non-finite or so small that its fp32 sum is dominated by subnormal rounding.
+constexpr float kCosMinNorm = 7.88860905e-31f; // 2^-100
+template <int DM> __device__ __forceinline__ float approx_eps(const ExactTcEps& e, float qn, float xn) {
+    const float a = sqrtf(qn), b = sqrtf(xn);
+    const float dot_err = e.rel * a * b + e.lin * (a + b) + e.abs;
+    if constexpr (DM == DM_COS) {
+        if (qn == 0.f || xn == 0.f) // both sides take the same zero-norm branch (0 or 1, exactly)
+            return e.rel + e.sum;
+        if (!(qn >= kCosMinNorm && xn >= kCosMinNorm && qn <= FLT_MAX && xn <= FLT_MAX))
+            return INFINITY;
+        return dot_err / (a * b) + e.sum; // plus norms, square roots, the division and the exact kernel's own sums
+    } else {
+        return 2.f * dot_err + e.sum * (qn + xn); // plus norms, the final sum and the exact kernel's own sum
+    }
 }
 
 template <int DM> __global__ void __launch_bounds__(kTcThreads, 1) exact_tc_filter_kernel(const __grid_constant__ TcParams p) {
@@ -291,7 +305,7 @@ template <int DM> __global__ void __launch_bounds__(kTcThreads, 1) exact_tc_filt
                         if (row < p.n) {
                             const float xn = __ldg(p.xn + row);
                             const float d = approx_distance<DM>(r[j], qn, xn);
-                            if (d < thr) {
+                            if (d < thr && d > -INFINITY) {
                                 // max-heap on the distance (root = the list's current worst, = thr once the list is full):
                                 // log2(KP) steps per accepted row.  A sorted array costs KP/2 shifts per insert, and every
                                 // insert of ANY lane stalls the whole warp.
@@ -306,7 +320,7 @@ template <int DM> __global__ void __launch_bounds__(kTcThreads, 1) exact_tc_filt
                                         pos = par;
                                     }
                                 } else { // replace the root; the evicted row is remembered through its lower bound
-                                    dropped = fminf(dropped, ld[0] - approx_eps<DM>(p.eps_rel, qn, __ldg(p.xn + li[0])));
+                                    dropped = fminf(dropped, ld[0] - approx_eps<DM>(p.eps, qn, __ldg(p.xn + li[0])));
                                     pos = 0;
                                     for (;;) {
                                         uint32_t c = 2 * pos + 1;
@@ -324,7 +338,10 @@ template <int DM> __global__ void __launch_bounds__(kTcThreads, 1) exact_tc_filt
                                 if (size == KP)
                                     thr = ld[0];
                             } else {
-                                dropped = fminf(dropped, d - approx_eps<DM>(p.eps_rel, qn, xn));
+                                // a NaN or infinite approximation bounds nothing (overflowed norms, NaN / inf components):
+                                // -inf makes the query unsafe
+                                const float lb = d - approx_eps<DM>(p.eps, qn, xn);
+                                dropped = lb < INFINITY ? fminf(dropped, lb) : -INFINITY;
                             }
                         }
                     }
@@ -360,7 +377,7 @@ struct RrParams {
     const float* xn;
     const float* qn;
     uint32_t groups, KP, k;
-    float eps_rel;
+    ExactTcEps eps;
     const float* cand_d;
     const uint32_t* cand_i;
     const float* dropped_lb;
@@ -370,7 +387,7 @@ struct RrParams {
     uint32_t* unsafe_count;
 };
 
-__device__ __forceinline__ bool closer_rr(float d, uint32_t id, float od, uint32_t oid) { return d < od || (d == od && id < oid); }
+__device__ __forceinline__ bool closer_rr(float d, uint32_t id, float od, uint32_t oid) { return closer_total(d, id, od, oid); }
 
 template <int DM> __global__ void __launch_bounds__(kRrThreads) exact_tc_rerank_kernel(const RrParams p) {
     extern __shared__ __align__(16) uint8_t sm_raw[];
@@ -395,7 +412,7 @@ template <int DM> __global__ void __launch_bounds__(kRrThreads) exact_tc_rerank_
     for (uint32_t i = threadIdx.x; i < P2; i += blockDim.x) {
         float u = INFINITY;
         if (i < C && ci[i] != 0xFFFFFFFFu)
-            u = cd[i] + approx_eps<DM>(p.eps_rel, qn, __ldg(p.xn + ci[i]));
+            u = cd[i] + approx_eps<DM>(p.eps, qn, __ldg(p.xn + ci[i]));
         ub[i] = u;
     }
     for (uint32_t c = threadIdx.x; c < p.nchunks; c += blockDim.x)
@@ -419,16 +436,19 @@ template <int DM> __global__ void __launch_bounds__(kRrThreads) exact_tc_rerank_
         kth_ub_s = p.k <= P2 ? ub[p.k - 1] : INFINITY; // +inf when fewer than k candidates exist: everything qualifies
     __syncthreads();
     const float kth_ub = kth_ub_s;
-    // anything a list dropped that could still qualify makes the query unsafe
-    for (uint32_t gI = threadIdx.x; gI < p.groups; gI += blockDim.x)
-        if (p.dropped_lb[(size_t)q * p.groups + gI] <= kth_ub)
+    // anything a list dropped that could still qualify makes the query unsafe (+inf: the list dropped nothing, which also
+    // holds when fewer than k candidates exist and kth_ub is +inf)
+    for (uint32_t gI = threadIdx.x; gI < p.groups; gI += blockDim.x) {
+        const float lb = p.dropped_lb[(size_t)q * p.groups + gI];
+        if (lb <= kth_ub && lb < INFINITY)
             bad = 1;
+    }
     // survivors
     for (uint32_t i = threadIdx.x; i < C; i += blockDim.x) {
         const uint32_t id = ci[i];
         if (id == 0xFFFFFFFFu)
             continue;
-        const float lb = cd[i] - approx_eps<DM>(p.eps_rel, qn, __ldg(p.xn + id));
+        const float lb = cd[i] - approx_eps<DM>(p.eps, qn, __ldg(p.xn + id));
         if (lb <= kth_ub) {
             const uint32_t at = atomicAdd(&nsel, 1u);
             if (at < kRrCap)
@@ -491,77 +511,135 @@ template <int DM> __global__ void __launch_bounds__(kRrThreads) exact_tc_rerank_
 
 } // namespace
 
+bool exact_tc_defined(int dist_mode, int scalar_kind, size_t n, size_t k) {
+    return scalar_kind == SK_F32 && (dist_mode == DM_L2SQ || dist_mode == DM_COS) && k <= 192 && n && n < 0xFFFFFFFFull;
+}
+
 bool exact_tc_applicable(int dist_mode, int scalar_kind, size_t n, size_t nq, size_t k, uint32_t row_bytes) {
     if (const char* e = getenv("LB200_EXACT")) {
         if (e[0] == 's') // "simt"
             return false;
         if (e[0] == 't') // "tc": force (still only where it is defined)
-            return scalar_kind == SK_F32 && (dist_mode == DM_L2SQ || dist_mode == DM_COS) && k <= 192 && n < 0xFFFFFFFFull && n && nq;
+            return exact_tc_defined(dist_mode, scalar_kind, n, k) && nq;
     }
     // the tensor-core pass pays off once the problem is a real GEMM
-    return scalar_kind == SK_F32 && (dist_mode == DM_L2SQ || dist_mode == DM_COS) && k <= 192 && n >= 32768 && n < 0xFFFFFFFFull &&
-           nq >= 16 && row_bytes >= 128;
+    return exact_tc_defined(dist_mode, scalar_kind, n, k) && n >= 32768 && nq >= 16 && row_bytes >= 128;
 }
 
-// Returns the device array of per-query "unsafe" flags (owned by the caller through `scratch`, freed with cudaFreeAsync by the
-// caller) so that launch_exact can run the SIMT kernels for exactly those queries.
-void launch_exact_tc(int dist_mode, const uint8_t* d_data, size_t n, size_t data_stride, const uint8_t* d_queries, size_t nq,
-                     size_t q_stride, uint32_t row_bytes, size_t k, uint64_t* d_keys, float* d_dists, uint8_t** d_unsafe,
-                     uint32_t** d_unsafe_count, cudaStream_t stream) {
+ExactTcPlan exact_tc_plan(size_t n, size_t nq, size_t k, uint32_t row_bytes) {
     const uint32_t nchunks = row_bytes / 16, dims = row_bytes / 4;
-    int sms = device_sm_count();
     const uint32_t q_tiles = (uint32_t)((nq + kTileM - 1) / kTileM);
     const uint32_t row_tiles = (uint32_t)((n + kTileN - 1) / kTileN);
-    uint32_t groups = std::max<uint32_t>(1, (uint32_t)sms / q_tiles);
-    groups = std::min(groups, row_tiles);
-    uint32_t KP = (uint32_t)round_up(k + std::max<size_t>(32, k / 2), 32);
-    KP = std::min(KP, kMaxKP);
-    const float eps_rel = (float)(dims + 32) * 5.9604645e-8f; // (dims + 32) * 2^-24
+    ExactTcPlan pl{};
+    pl.KP = std::min<uint32_t>((uint32_t)round_up(k + std::max<size_t>(32, k / 2), 32), kMaxKP);
+    pl.groups = std::min(std::max<uint32_t>(1, (uint32_t)device_sm_count() / q_tiles), row_tiles);
+    // The re-rank bitonic-sorts next_pow2(groups * KP) upper bounds in shared memory.  With one query tile on a 132-SM H100
+    // SXM and KP = 256 (k >= 150) that is 65536 floats, over the 227 KB opt-in limit; capping groups at 128 (4 SMs idle in
+    // that case only) keeps the filter's occupancy and the sort's cost.
+    int dev = 0, optin = 0;
+    LB_CUDA(cudaGetDevice(&dev));
+    LB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    cudaFuncAttributes fa_cos{}, fa_l2{}; // the dynamic request may use what the kernel's static __shared__ leaves
+    LB_CUDA(cudaFuncGetAttributes(&fa_cos, exact_tc_rerank_kernel<DM_COS>));
+    LB_CUDA(cudaFuncGetAttributes(&fa_l2, exact_tc_rerank_kernel<DM_L2SQ>));
+    const size_t rr_static = std::max(fa_cos.sharedSizeBytes, fa_l2.sharedSizeBytes);
+    size_t p2max = 1;
+    while ((p2max * 2) * 4 + (size_t)kRrCap * 8 + row_bytes + rr_static <= (size_t)optin)
+        p2max *= 2;
+    pl.groups = std::max<uint32_t>(1, std::min<uint32_t>(pl.groups, (uint32_t)(p2max / pl.KP)));
+    // |approx - exact| where u = 2^-24, L = chunks per lane and both sides are fp32:
+    //  rel  3xTF32 drops lo*lo and lo's own rounding (3 * 2^-22 |q_i x_i|) and accumulates 3 dims / 8 MMAs into fp32 (about
+    //       dims u with truncating adds): (dims + 32) u |q||x|
+    //  sum  every fp32 sum here (norms_kernel, exact.cu's sum of (q-x)^2 or of q.x and |x|^2) rounds a term at most L + 9
+    //       times (4 inside a chunk, L along the lane, 5 in the butterfly); with the exact distance <= 2 (|q|^2 + |x|^2)
+    //       and the final two operations that is (3 L + 29) u (|q|^2 + |x|^2) for l2sq, about (3 L + 33) u for cos.
+    //       (3 L + 48) u keeps 3e-6 at L = 1.
+    //  lin, abs  the tensor cores may flush subnormal inputs, products and partial sums, each below 2^-126:
+    //       2^-126 (sqrt(dims) (|q| + |x|) + 6 dims) with the two sides' subnormal roundings, rounded up to 8 dims
+    const uint32_t L = (nchunks + 31) / 32;
+    const float u = 5.9604645e-8f, tiny = 1.17549435e-38f; // 2^-24, 2^-126
+    pl.eps.rel = (float)(dims + 32) * u;
+    pl.eps.sum = (float)(3 * L + 48) * u;
+    pl.eps.lin = sqrtf((float)dims) * tiny;
+    pl.eps.abs = (float)(8 * dims) * tiny;
+    return pl;
+}
+
+// Returns the device array of per-query "unsafe" flags (owned by the caller, freed with cudaFreeAsync by the caller) so that
+// launch_exact can run the SIMT kernels for exactly those queries.  On an error everything it allocated is freed.
+void launch_exact_tc(int dist_mode, const uint8_t* d_data, size_t n, size_t data_stride, const uint8_t* d_queries, size_t nq,
+                     size_t q_stride, uint32_t row_bytes, size_t k, uint64_t* d_keys, float* d_dists, uint8_t** d_unsafe,
+                     uint32_t** d_unsafe_count, cudaStream_t stream, const ExactTcProbe* probe) {
+    const uint32_t nchunks = row_bytes / 16;
+    const ExactTcPlan pl = exact_tc_plan(n, nq, k, row_bytes);
+    const uint32_t groups = pl.groups, KP = pl.KP;
+    const uint32_t q_tiles = (uint32_t)((nq + kTileM - 1) / kTileM);
+    const uint32_t row_tiles = (uint32_t)((n + kTileN - 1) / kTileN);
 
     float *xn = nullptr, *qn = nullptr, *cand_d = nullptr, *dropped = nullptr;
     uint32_t* cand_i = nullptr;
-    LB_CUDA(cudaMallocAsync(&xn, n * sizeof(float), stream));
-    LB_CUDA(cudaMallocAsync(&qn, nq * sizeof(float), stream));
-    LB_CUDA(cudaMallocAsync(&cand_d, nq * groups * KP * sizeof(float), stream));
-    LB_CUDA(cudaMallocAsync(&cand_i, nq * groups * KP * sizeof(uint32_t), stream));
-    LB_CUDA(cudaMallocAsync(&dropped, nq * groups * sizeof(float), stream));
-    LB_CUDA(cudaMallocAsync(d_unsafe, nq, stream));
-    LB_CUDA(cudaMallocAsync(d_unsafe_count, sizeof(uint32_t), stream));
-    LB_CUDA(cudaMemsetAsync(*d_unsafe_count, 0, sizeof(uint32_t), stream));
-    norms_kernel<<<(unsigned)((n + 7) / 8), 256, 0, stream>>>(d_data, n, data_stride, nchunks, xn);
-    norms_kernel<<<(unsigned)((nq + 7) / 8), 256, 0, stream>>>(d_queries, nq, q_stride, nchunks, qn);
-    count_launch(2);
-
-    TcParams p{};
-    p.data = d_data, p.n = n, p.data_stride = data_stride;
-    p.queries = d_queries, p.nq = (uint32_t)nq, p.q_stride = q_stride, p.nchunks = nchunks;
-    p.xn = xn, p.qn = qn, p.groups = groups, p.row_tiles = row_tiles, p.KP = KP, p.eps_rel = eps_rel;
-    p.cand_d = cand_d, p.cand_i = cand_i, p.dropped_lb = dropped;
-    RrParams r{};
-    r.data = d_data, r.n = n, r.data_stride = data_stride, r.queries = d_queries, r.nq = (uint32_t)nq, r.q_stride = q_stride;
-    r.nchunks = nchunks, r.xn = xn, r.qn = qn, r.groups = groups, r.KP = KP, r.k = (uint32_t)k, r.eps_rel = eps_rel;
-    r.cand_d = cand_d, r.cand_i = cand_i, r.dropped_lb = dropped, r.out_keys = d_keys, r.out_dists = d_dists;
-    r.unsafe = *d_unsafe, r.unsafe_count = *d_unsafe_count;
-    uint32_t P2 = 1;
-    while (P2 < groups * KP)
-        P2 <<= 1;
-    const size_t rr_smem = (size_t)P2 * 4 + (size_t)kRrCap * 8 + row_bytes;
-    auto run = [&](auto dm) {
-        constexpr int DM = decltype(dm)::value;
-        auto fk = exact_tc_filter_kernel<DM>;
-        LB_CUDA(cudaFuncSetAttribute(fk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem));
-        fk<<<q_tiles * groups, kTcThreads, kTcSmem, stream>>>(p);
-        LB_CUDA(cudaGetLastError());
-        auto rk = exact_tc_rerank_kernel<DM>;
-        LB_CUDA(cudaFuncSetAttribute(rk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rr_smem));
-        rk<<<(unsigned)nq, kRrThreads, rr_smem, stream>>>(r);
-        LB_CUDA(cudaGetLastError());
+    *d_unsafe = nullptr, *d_unsafe_count = nullptr;
+    try {
+        LB_CUDA(cudaMallocAsync(&xn, n * sizeof(float), stream));
+        LB_CUDA(cudaMallocAsync(&qn, nq * sizeof(float), stream));
+        LB_CUDA(cudaMallocAsync(&cand_d, nq * groups * KP * sizeof(float), stream));
+        LB_CUDA(cudaMallocAsync(&cand_i, nq * groups * KP * sizeof(uint32_t), stream));
+        LB_CUDA(cudaMallocAsync(&dropped, nq * groups * sizeof(float), stream));
+        LB_CUDA(cudaMallocAsync(d_unsafe, nq, stream));
+        LB_CUDA(cudaMallocAsync(d_unsafe_count, sizeof(uint32_t), stream));
+        LB_CUDA(cudaMemsetAsync(*d_unsafe_count, 0, sizeof(uint32_t), stream));
+        norms_kernel<<<(unsigned)((n + 7) / 8), 256, 0, stream>>>(d_data, n, data_stride, nchunks, xn);
+        norms_kernel<<<(unsigned)((nq + 7) / 8), 256, 0, stream>>>(d_queries, nq, q_stride, nchunks, qn);
         count_launch(2);
-    };
-    if (dist_mode == DM_COS)
-        run(std::integral_constant<int, DM_COS>{});
-    else
-        run(std::integral_constant<int, DM_L2SQ>{});
+
+        TcParams p{};
+        p.data = d_data, p.n = n, p.data_stride = data_stride;
+        p.queries = d_queries, p.nq = (uint32_t)nq, p.q_stride = q_stride, p.nchunks = nchunks;
+        p.xn = xn, p.qn = qn, p.groups = groups, p.row_tiles = row_tiles, p.KP = KP, p.eps = pl.eps;
+        p.cand_d = cand_d, p.cand_i = cand_i, p.dropped_lb = dropped;
+        RrParams r{};
+        r.data = d_data, r.n = n, r.data_stride = data_stride, r.queries = d_queries, r.nq = (uint32_t)nq, r.q_stride = q_stride;
+        r.nchunks = nchunks, r.xn = xn, r.qn = qn, r.groups = groups, r.KP = KP, r.k = (uint32_t)k, r.eps = pl.eps;
+        r.cand_d = cand_d, r.cand_i = cand_i, r.dropped_lb = dropped, r.out_keys = d_keys, r.out_dists = d_dists;
+        r.unsafe = *d_unsafe, r.unsafe_count = *d_unsafe_count;
+        uint32_t P2 = 1;
+        while (P2 < groups * KP)
+            P2 <<= 1;
+        const size_t rr_smem = (size_t)P2 * 4 + (size_t)kRrCap * 8 + row_bytes;
+        auto run = [&](auto dm) {
+            constexpr int DM = decltype(dm)::value;
+            auto fk = exact_tc_filter_kernel<DM>;
+            LB_CUDA(cudaFuncSetAttribute(fk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem));
+            fk<<<q_tiles * groups, kTcThreads, kTcSmem, stream>>>(p);
+            LB_CUDA(cudaGetLastError());
+            auto rk = exact_tc_rerank_kernel<DM>;
+            LB_CUDA(cudaFuncSetAttribute(rk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rr_smem));
+            rk<<<(unsigned)nq, kRrThreads, rr_smem, stream>>>(r);
+            LB_CUDA(cudaGetLastError());
+            count_launch(2);
+        };
+        if (dist_mode == DM_COS)
+            run(std::integral_constant<int, DM_COS>{});
+        else
+            run(std::integral_constant<int, DM_L2SQ>{});
+        if (probe) {
+            const size_t nc = nq * groups * KP;
+            LB_CUDA(cudaMemcpyAsync(probe->qn, qn, nq * sizeof(float), cudaMemcpyDeviceToHost, stream));
+            LB_CUDA(cudaMemcpyAsync(probe->xn, xn, n * sizeof(float), cudaMemcpyDeviceToHost, stream));
+            LB_CUDA(cudaMemcpyAsync(probe->cand_d, cand_d, nc * sizeof(float), cudaMemcpyDeviceToHost, stream));
+            LB_CUDA(cudaMemcpyAsync(probe->cand_i, cand_i, nc * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+            LB_CUDA(cudaMemcpyAsync(probe->dropped_lb, dropped, nq * groups * sizeof(float), cudaMemcpyDeviceToHost, stream));
+            LB_CUDA(cudaMemcpyAsync(probe->unsafe, *d_unsafe, nq, cudaMemcpyDeviceToHost, stream));
+            LB_CUDA(cudaStreamSynchronize(stream));
+        }
+    } catch (...) {
+        (void)cudaGetLastError(); // a refused launch configuration must not fail the caller's next, unrelated launch
+        for (void* b : {(void*)xn, (void*)qn, (void*)cand_d, (void*)cand_i, (void*)dropped, (void*)*d_unsafe, (void*)*d_unsafe_count})
+            if (b)
+                cudaFreeAsync(b, stream);
+        *d_unsafe = nullptr, *d_unsafe_count = nullptr;
+        throw;
+    }
     LB_CUDA(cudaFreeAsync(xn, stream));
     LB_CUDA(cudaFreeAsync(qn, stream));
     LB_CUDA(cudaFreeAsync(cand_d, stream));

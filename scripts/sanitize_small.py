@@ -44,6 +44,9 @@ os.environ["LB200_EXACT"] = "simt"
 ks, ds = api.exact_search(X, Q, k, "l2sq")
 os.environ.pop("LB200_EXACT")
 assert np.array_equal(kt, ks) and np.array_equal(dt.view(np.uint32), ds.view(np.uint32))
+# the same through the filter's test hook, which copies its intermediate buffers out
+pr = api.exact_tc_probe(X, Q, k, "cos")
+assert not pr["unsafe"].any()
 # the warp-per-query kernel alone and as a two-rank group on one device (owner + helper pool, mailboxes, fused all-gather)
 g = api.Index(d, "cos", "f32", M=8, efc=32, ef=24)
 g.reserve(n)
