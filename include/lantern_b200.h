@@ -108,10 +108,13 @@ typedef struct lb200_search_stats_t {
     uint64_t computed_distances; /* == usearch search_result_t::computed_distances summed over the batch */
     uint64_t base_pops;          /* level-0 candidates expanded */
     uint64_t upper_hops;         /* level>=1 neighbour lists scanned */
-    uint64_t algorithmic_bytes;  /* computed_distances*row_bytes + (base_pops*(4+4*M0) + upper_hops*(4+4*M)) + queries*row_bytes */
+    uint64_t algorithmic_bytes;  /* full_rows_read*row_bytes + screened candidates*(code row + 16) + (base_pops*(4+4*M0) +
+                                    upper_hops*(4+4*M)) + queries*row_bytes: the bytes the search needed */
     double kernel_ms;            /* device time of the search kernel alone (CUDA events on the launching stream) */
     uint64_t limbo_overflows;    /* equal-distance candidates beyond the 64 the walker parks at the eviction boundary (only
                                     possible with massive exact ties; each one may be an expansion the reference performs) */
+    uint64_t full_rows_read;     /* (appended field) stored rows read in full: computed_distances minus the candidates the
+                                    int8 screen of f32 l2sq / cos searches rejected from their codes alone */
 } lb200_search_stats_t;
 
 /* Work of the most recent lb200_build (or implicit build): the build metric of SURVEY.md 8d is
@@ -237,6 +240,12 @@ LB200_EXPORT void lb200_exact_tc_probe(float const* dataset, size_t dataset_size
                                        float* eps, float* qn, float* xn, float* cand_d, uint32_t* cand_i, float* dropped_lb,
                                        uint8_t* unsafe, lb200_key_t* keys, lb200_distance_t* distances,
                                        lb200_error_t* error);
+/* Test hook, not a search entry point: for every (query, row) pair of dense f32 rows (l2sq or cos), the search screen's lower
+ * bound lb[queries_size][dataset_size] and the search kernel's own fp32 distance d[queries_size][dataset_size], computed
+ * by the device functions the search uses (the rows are encoded as an index encodes them); lb <= d must hold. */
+LB200_EXPORT void lb200_search_screen_probe(float const* dataset, size_t dataset_size, float const* queries, size_t queries_size,
+                                            size_t dimensions, lb200_metric_kind_t metric_kind, float* lb, float* d,
+                                            lb200_error_t* error);
 /* f32 -> f16 / i8 / b1 (index_plugins.hpp:879-974); host memory; `count` vectors. */
 LB200_EXPORT void lb200_cast(lb200_scalar_kind_t from, void const* vectors, lb200_scalar_kind_t to, void* result,
                              size_t result_size, int dims, lb200_error_t* error);

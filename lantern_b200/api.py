@@ -55,7 +55,7 @@ class IndexMetadata(C.Structure):  # == usearch_index_metadata_t (usearch.h:119-
 class SearchStats(C.Structure):
     _fields_ = [("queries", C.c_uint64), ("computed_distances", C.c_uint64), ("base_pops", C.c_uint64),
                 ("upper_hops", C.c_uint64), ("algorithmic_bytes", C.c_uint64), ("kernel_ms", C.c_double),
-                ("limbo_overflows", C.c_uint64)]
+                ("limbo_overflows", C.c_uint64), ("full_rows_read", C.c_uint64)]
 
 
 class BuildStats(C.Structure):
@@ -125,6 +125,8 @@ SIGNATURES = {
     "lb200_exact_tc_probe": (None, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_size_t,
                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_void_p, ERRP]),
+    "lb200_search_screen_probe": (None, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_void_p,
+                                         C.c_void_p, ERRP]),
     "lb200_cast": (None, [C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_int, ERRP]),
     "lb200_cast_batch": (None, [C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_void_p, ERRP]),
     "lb200_quantize_pq": (None, [C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
@@ -462,6 +464,16 @@ def exact_tc_probe(dataset, queries, k, metric="l2sq"):
     _static("lb200_exact_tc_probe", *args, *(_ptr(out[f]) for f in ("qn", "xn", "cand_d", "cand_i", "dropped_lb", "unsafe",
                                                                      "keys", "dists")))
     return out
+
+
+def search_screen_probe(dataset, queries, metric="l2sq"):
+    """Test hook: (lb, d), both [nq][n] float32 -- the search screen's lower bound and the search kernel's fp32 distance."""
+    X = np.ascontiguousarray(dataset, dtype=np.float32)
+    Q = np.ascontiguousarray(queries, dtype=np.float32)
+    lb = np.zeros((len(Q), len(X)), np.float32)
+    d = np.zeros((len(Q), len(X)), np.float32)
+    _static("lb200_search_screen_probe", _ptr(X), len(X), _ptr(Q), len(Q), X.shape[1], METRIC[metric], _ptr(lb), _ptr(d))
+    return lb, d
 
 
 def cast(vectors_f32, quant):

@@ -323,6 +323,7 @@ LB200_EXPORT void lb200_last_search_stats(lb200_index_t h, lb200_search_stats_t*
         stats->algorithmic_bytes = s.algorithmic_bytes;
         stats->kernel_ms = s.kernel_ms;
         stats->limbo_overflows = s.limbo_overflows;
+        stats->full_rows_read = s.full_rows_read;
     });
 }
 
@@ -559,6 +560,27 @@ LB200_EXPORT void lb200_exact_tc_probe(float const* dataset, size_t dataset_size
                      dk.as<uint64_t>(), dv.as<float>(), 0, &probe);
         LB_CUDA(cudaMemcpy(keys, dk.p, queries_size * count * 8, cudaMemcpyDeviceToHost));
         LB_CUDA(cudaMemcpy(distances, dv.p, queries_size * count * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+LB200_EXPORT void lb200_search_screen_probe(float const* dataset, size_t dataset_size, float const* queries, size_t queries_size,
+                                            size_t dimensions, lb200_metric_kind_t metric_kind, float* lb, float* d,
+                                            lb200_error_t* error) {
+    guarded(error, [&] {
+        require_device();
+        check_metric_scalar(metric_kind, lb200_scalar_f32_k);
+        const int dm = distance_mode(metric_kind, SK_F32);
+        if ((dm != DM_L2SQ && dm != DM_COS) || !dimensions || !lb || !d)
+            throw CudaError("search_screen_probe: needs l2sq or cos, dimensions and output buffers");
+        if (!dataset_size || !queries_size)
+            return;
+        const size_t rb = round_up(dimensions * 4, 16);
+        DeviceTemp dd(dataset_size * rb), dq(queries_size * rb), dl(queries_size * dataset_size * 4), dv(queries_size * dataset_size * 4);
+        upload_rows(dataset, dataset_size, dimensions * 4, SK_F32, dimensions, dd.as<uint8_t>(), rb);
+        upload_rows(queries, queries_size, dimensions * 4, SK_F32, dimensions, dq.as<uint8_t>(), rb);
+        launch_screen_probe(dm, dd.as<uint8_t>(), dataset_size, dq.as<uint8_t>(), queries_size, (uint32_t)rb, dl.as<float>(), dv.as<float>(), 0);
+        LB_CUDA(cudaMemcpy(lb, dl.p, queries_size * dataset_size * 4, cudaMemcpyDeviceToHost));
+        LB_CUDA(cudaMemcpy(d, dv.p, queries_size * dataset_size * 4, cudaMemcpyDeviceToHost));
     });
 }
 

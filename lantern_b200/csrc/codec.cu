@@ -12,6 +12,7 @@
 #include <cuda_fp16.h>
 
 #include "engine.h"
+#include "screen.cuh"
 
 namespace lb200 {
 
@@ -198,7 +199,80 @@ __global__ void pq_query_tables_kernel(const float* __restrict__ codebook, uint3
     }
 }
 
+// Companion int8 copy of stored f32 rows for the search screen (screen.cuh, DESIGN.md 4.1).  One warp per row:
+//   codes: c_i = clamp(round(x_i / s), -127, 127), s = max|x_i| / 127 (fp32), word w = dims 4w..4w+3, zero padded;
+//   meta:  {s, r >= |x - s c| (double, rounded up), b2 = |x|^2 exactly as the search kernel computes it, |c| rounded up}.
+// Rows holding NaN / inf, or whose scale underflows to 0, get r = +inf: their bound is -inf and they always pass.
+__global__ void sq_encode_kernel(const uint8_t* __restrict__ rows, uint32_t row_bytes, size_t n, uint8_t* __restrict__ codes,
+                                 uint32_t code_bytes, float4* __restrict__ meta) {
+    const size_t row = (size_t)blockIdx.x * (blockDim.x / 32) + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (row >= n)
+        return;
+    const uint4* x = reinterpret_cast<const uint4*>(rows + row * row_bytes);
+    const uint32_t nchunks = row_bytes / 16;
+    // |x|^2 with accum_chunk<DM_COS, SK_F32> + finish_distance's fold, chunk for chunk in the kernel's order: the same bits
+    DistAcc<DM_COS, SK_F32> acc;
+    acc.reset();
+    const uint4 zero = make_uint4(0, 0, 0, 0);
+    float amax = 0.f;
+    bool finite = true;
+    for (uint32_t c = lane; c < nchunks; c += 32) {
+        const uint4 v = x[c];
+        accum_chunk<DM_COS, SK_F32>(acc, zero, v);
+        const float f[4] = {__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w)};
+#pragma unroll
+        for (int b = 0; b < 4; ++b)
+            finite = finite && isfinite(f[b]), amax = fmaxf(amax, fabsf(f[b]));
+    }
+    const float b2 = warp_sum(acc.v[2] + acc.v[3]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1)
+        amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    finite = __all_sync(0xffffffffu, finite);
+    const float scale = (float)((double)amax / 127.0);
+    const bool ok = finite && (amax == 0.f || scale > 0.f);
+    double e2 = 0.0;
+    uint32_t c2 = 0;
+    uint32_t* out = reinterpret_cast<uint32_t*>(codes + row * code_bytes);
+    for (uint32_t w = lane; w < code_bytes / 4; w += 32) {
+        uint32_t word = 0;
+        if (w < nchunks && ok && scale > 0.f) {
+            const uint4 v = x[w];
+            const float f[4] = {__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w)};
+#pragma unroll
+            for (int b = 0; b < 4; ++b) {
+                const int ci = (int)fmin(fmax(rint((double)f[b] / (double)scale), -127.0), 127.0);
+                const double e = (double)f[b] - (double)scale * (double)ci; // s * c is exact in double
+                e2 += e * e, c2 += (uint32_t)(ci * ci);
+                word |= (uint32_t)(uint8_t)(int8_t)ci << (8 * b);
+            }
+        }
+        out[w] = word;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        e2 += __shfl_xor_sync(0xffffffffu, e2, o);
+        c2 += __shfl_xor_sync(0xffffffffu, c2, o);
+    }
+    if (lane == 0) {
+        // < 80 double roundings of non-negative terms in e2: relative 2^-46; 2^-40 and the final 2^-50 cover them and the sqrt
+        const float r = ok ? __double2float_ru(sqrt(e2 * (1.0 + 0x1p-40)) * (1.0 + 0x1p-50)) : INFINITY;
+        meta[row] = make_float4(ok ? scale : 0.f, r, b2, __double2float_ru(sqrt((double)c2) * (1.0 + 0x1p-50)));
+    }
+}
+
 } // namespace
+
+void launch_sq_encode(const uint8_t* d_rows, size_t row_bytes, size_t n, uint8_t* d_codes, float4* d_meta, cudaStream_t stream) {
+    if (!n)
+        return;
+    const int warps = 8;
+    sq_encode_kernel<<<(unsigned)((n + warps - 1) / warps), warps * 32, 0, stream>>>(
+        d_rows, (uint32_t)row_bytes, n, d_codes, screen_code_bytes((uint32_t)row_bytes), d_meta);
+    LB_CUDA(cudaGetLastError());
+    count_launch();
+}
 
 void launch_pq_query_tables(const float* d_codebook, size_t dims, size_t nsub, size_t lut_width, bool cosine, const float* d_queries,
                             size_t q_stride_floats, size_t nq, float* d_tables, cudaStream_t stream) {

@@ -11,11 +11,14 @@
 #include <algorithm>
 
 #include "distance.cuh"
+#include "screen.cuh"
 
 namespace lb200 {
 
 // rows up to this many bytes are searched by the warp-per-query kernel unless "search_kernel" says otherwise (0: never)
 constexpr size_t kWarpKernelMaxRowBytes = 0;
+// rows of at least this many bytes take the screened search path when the index keeps the int8 companion
+constexpr size_t kScreenMinRowBytes = 1024;
 
 std::atomic<uint64_t> g_kernel_launches{0};
 
@@ -78,6 +81,8 @@ Index::Index(const IndexConfig& cfg, const float* codebook) : cfg_(cfg) {
     } else {
         stored_bytes_ = vec_bytes_;
         row_bytes_ = round_up(vec_bytes_, 16);
+        if (cfg.scalar_kind == SK_F32 && (dist_mode_ == DM_L2SQ || dist_mode_ == DM_COS))
+            sq_bytes_ = screen_code_bytes((uint32_t)row_bytes_);
     }
     LB_CUDA(cudaMalloc(&scratch_.counters, 8 * sizeof(unsigned long long)));
     LB_CUDA(cudaMemset(scratch_.counters, 0, 8 * sizeof(unsigned long long)));
@@ -90,6 +95,7 @@ Index::~Index() {
     cudaFree(d_codebook_), cudaFree(scratch_.visited), cudaFree(scratch_.touched), cudaFree(scratch_.counters);
     cudaFree(d_query_buf_), cudaFree(d_io_buf_), cudaFree(d_warp_aux_);
     cudaFree(d_pq_pair_), cudaFree(d_pq_norm_), cudaFree(d_pending_raw_), cudaFree(d_pq_tables_);
+    cudaFree(d_sq_codes_), cudaFree(d_sq_meta_);
     if (ev0_)
         cudaEventDestroy(ev0_);
     if (ev1_)
@@ -106,7 +112,16 @@ void Index::ensure_capacity(size_t cap) {
     grow_device(d_adj0_, n_ * cfg_.M0, nc * cfg_.M0, 0xFF);
     grow_device(d_upper_ref_, n_, nc, 0xFF);
     grow_device(d_keys_, n_, nc, 0xFF);
+    if (sq_bytes_) {
+        grow_device(d_sq_codes_, used * sq_bytes_, nc * sq_bytes_, 0);
+        grow_device(d_sq_meta_, used, nc, 0);
+    }
     capacity_ = nc;
+}
+
+void Index::encode_screen(size_t first, size_t count) {
+    if (sq_bytes_)
+        launch_sq_encode(d_vectors_ + first * row_bytes_, row_bytes_, count, d_sq_codes_ + first * sq_bytes_, d_sq_meta_ + first, 0);
 }
 
 void Index::reserve(size_t capacity) {
@@ -186,6 +201,7 @@ void Index::add_device(const uint64_t* host_keys, const void* d_vectors, size_t 
         launch_cast_rows(d_vectors, stride, SK_F32, (uint8_t*)d_pending_raw_ + pending_n_ * raw_row, raw_row, SK_F32, cfg_.dims, n, 0);
     } else {
         launch_cast_rows(d_vectors, stride, kind, d_vectors_ + used * row_bytes_, row_bytes_, cfg_.scalar_kind, cfg_.dims, n, 0);
+        encode_screen(used, n);
     }
     h_keys_.insert(h_keys_.end(), host_keys, host_keys + n);
     pending_n_ += n;
@@ -282,6 +298,8 @@ GraphView Index::view() const {
     // the reference's encoder never emits centroid ids >= 128 (signed-char loop, lantern_storage.hpp:123) and neither does
     // lb200_add*: then half of a 256-entry table can never be addressed and is not built (half the shared memory)
     g.pq_lut_width = (uint32_t)((cfg_.num_centroids > 128 && pq_max_code_ < 128) ? 128 : cfg_.num_centroids);
+    g.sq_codes = d_sq_codes_;
+    g.sq_meta = d_sq_meta_;
     g.flags = 2u; // L2-prefetch the adjacency line of nodes that enter the top list
     if (const char* e = getenv("LB200_FLAGS"))
         g.flags = (uint32_t)atoi(e);
@@ -342,6 +360,7 @@ void Index::search_device(const void* d_queries, size_t nq, size_t stride, int k
         launch_warp_search(*this, qbuf, qrow, nq, k, (uint32_t)L, d_keys, d_dists, d_counts, stream);
         LB_CUDA(cudaEventRecord(ev1_, stream));
         last_nq_ = (uint32_t)nq;
+        last_screened_ = false;
         return;
     }
     GraphView gv = view();
@@ -362,7 +381,12 @@ void Index::search_device(const void* d_queries, size_t nq, size_t stride, int k
             gv.pq_query_tables = d_pq_tables_;
         }
     }
-    const uint32_t max_ctas = search_max_ctas(dist_mode_, cfg_.scalar_kind, gv, (uint32_t)L, cfg_.pq, expand);
+    // int8 screen of the level-0 beam (screen.cuh): below 1 KB per row the extra dependent fetch per round is unlikely to pay
+    // for the bytes it saves.  LB200_SEARCH_SCREEN=0/1 overrides the choice for experiments (same graph timed both ways).
+    bool screen = sq_bytes_ && row_bytes_ >= kScreenMinRowBytes;
+    if (const char* e = getenv("LB200_SEARCH_SCREEN"))
+        screen = sq_bytes_ && atoi(e) != 0;
+    const uint32_t max_ctas = search_max_ctas(dist_mode_, cfg_.scalar_kind, gv, (uint32_t)L, cfg_.pq, expand, screen);
     ensure_scratch(max_ctas);
     LB_CUDA(cudaMemsetAsync(scratch_.counters, 0, 8 * sizeof(unsigned long long), stream));
 
@@ -374,11 +398,13 @@ void Index::search_device(const void* d_queries, size_t nq, size_t stride, int k
     p.query_stride = (uint32_t)qrow;
     p.nq = (uint32_t)nq, p.k = (uint32_t)k, p.L = (uint32_t)L;
     p.expand = expand;
+    p.screen = screen;
     p.out_keys = d_keys, p.out_dists = d_dists, p.out_counts = d_counts;
     LB_CUDA(cudaEventRecord(ev0_, stream));
     launch_search(dist_mode_, cfg_.scalar_kind, cfg_.pq, p, stream);
     LB_CUDA(cudaEventRecord(ev1_, stream));
     last_nq_ = (uint32_t)nq;
+    last_screened_ = screen;
 }
 
 void Index::search_host(const void* queries, size_t nq, size_t stride, int kind, size_t k, size_t ef, uint64_t* keys,
@@ -431,9 +457,12 @@ SearchStats Index::last_stats() {
             (void)cudaGetLastError();
     }
     s.computed_distances = c[1], s.base_pops = c[2], s.upper_hops = c[3], s.limbo_overflows = c[4];
-    // SURVEY.md 8(d): B_alg = n_dist*bytes_per_stored_vector + n_pop*(4 + M_level*4) + query bytes
-    s.algorithmic_bytes = s.computed_distances * (cfg_.pq ? stored_bytes_ : vec_bytes_) + s.base_pops * (4 + 4 * cfg_.M0) +
-                          s.upper_hops * (4 + 4 * cfg_.M) + s.queries * vec_bytes_;
+    const uint64_t screened = last_screened_ ? c[5] : 0, rejected = last_screened_ ? c[6] : 0;
+    s.full_rows_read = s.computed_distances - rejected;
+    // SURVEY.md 8(d): B_alg = n_dist*bytes_per_stored_vector + n_pop*(4 + M_level*4) + query bytes, where a screened search
+    // reads a code row + its 16 bytes of metadata per screened candidate and a stored row only for the rest
+    s.algorithmic_bytes = screened * (sq_bytes_ + 16) + s.full_rows_read * (cfg_.pq ? stored_bytes_ : vec_bytes_) +
+                          s.base_pops * (4 + 4 * cfg_.M0) + s.upper_hops * (4 + 4 * cfg_.M) + s.queries * vec_bytes_;
     return s;
 }
 

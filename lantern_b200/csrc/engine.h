@@ -9,6 +9,8 @@
 //                                     level-1 list; level l list at (ref + l-1)*M
 //   upper_adj [sum(levels)*M] u32     padded with 0xFFFFFFFF
 //   keys      [capacity] u64, levels [capacity] i16
+//   sq_codes  [capacity][round_up(dims,16)] i8   f32 l2sq / cos only: the search screen's int8 copy of every row (screen.cuh)
+//   sq_meta   [capacity] float4                  {scale, bound on |x - x^|, fp32 |x|^2 as the kernel computes it, |codes|}
 //   scratch   per resident CTA: visited bitmap (capacity bits) + touched-word list
 // The reference keeps the same information in per-node byte tapes with 6-byte slots
 // (U/include/usearch/index.hpp:1799-1863); only the (de)serialiser here speaks that format.
@@ -35,6 +37,7 @@ struct IndexConfig {
 
 struct SearchStats {
     uint64_t queries = 0, computed_distances = 0, base_pops = 0, upper_hops = 0, algorithmic_bytes = 0, limbo_overflows = 0;
+    uint64_t full_rows_read = 0; // stored rows actually read: computed_distances minus the candidates the screen rejected
     double kernel_ms = 0; // device time of the search kernel alone (CUDA events on the launching stream)
 };
 
@@ -58,12 +61,16 @@ struct GraphView {
     uint32_t flags;        // tuning: 1 = L2-prefetch the adjacency of every measured node, 2 = of accepted nodes only
     uint32_t dims, num_centroids, num_subvectors;
     uint32_t pq_lut_width; // centroids the per-value table covers (= num_centroids, or 128 when every stored code is < 128)
+    // search screen (f32 l2sq / cos): int8 code rows of screen_code_bytes(row_bytes) and their metadata, or NULL
+    const uint8_t* sq_codes;
+    const float4* sq_meta;
 };
 
 struct SearchScratch {
     uint32_t* visited;     // [ctas][words_per_cta]
     uint32_t* touched;     // [ctas][touched_cap]
-    unsigned long long* counters; // [0]=next query, [1]=dist evals, [2]=base pops, [3]=upper hops, [4]=limbo overflows (8 slots)
+    unsigned long long* counters; // [0]=next query, [1]=dist evals, [2]=base pops, [3]=upper hops, [4]=limbo overflows,
+                                  // [5]=candidates screened, [6]=candidates the screen rejected (8 slots)
     size_t words_per_cta;
     uint32_t touched_cap;
     uint32_t ctas;
@@ -143,6 +150,11 @@ class Index {
     size_t pq_tables_bytes_ = 0;
     uint32_t pq_max_code_ = 0; // largest centroid id present in the stored codes
     float* d_pending_raw_ = nullptr; // pq: raw f32 rows of the pending vectors (the value side of build distances)
+    // search screen companion (f32 storage, l2sq / cos, not PQ): written from d_vectors_ by launch_sq_encode
+    uint8_t* d_sq_codes_ = nullptr;
+    float4* d_sq_meta_ = nullptr;
+    size_t sq_bytes_ = 0; // bytes of one code row; 0 = this index keeps no companion
+    bool last_screened_ = false;
     size_t pending_raw_cap_ = 0;
     // host mirrors of the small per-node metadata
     std::vector<int16_t> h_levels_;
@@ -172,6 +184,7 @@ class Index {
     std::mutex stream_mu_;
 
     void ensure_scratch(uint32_t ctas);
+    void encode_screen(size_t first, size_t count); // companion of rows [first, first + count) from d_vectors_
     void* io_buffer(size_t bytes);
     uint8_t* query_buffer(size_t bytes);
 };
@@ -188,6 +201,8 @@ void launch_pq_tables(const float* d_codebook, size_t dims, size_t ncent, size_t
 // per-query ADC tables of a batch: out[q][s * lut_width + c] (+ |q|^2 at [nsub * lut_width]), row stride = nsub*lut_width + 4 floats
 void launch_pq_query_tables(const float* d_codebook, size_t dims, size_t nsub, size_t lut_width, bool cosine, const float* d_queries,
                             size_t q_stride_floats, size_t nq, float* d_tables, cudaStream_t stream);
+// screen.cuh companion of n stored f32 rows (row_bytes apart): codes[n][screen_code_bytes(row_bytes)], meta[n]
+void launch_sq_encode(const uint8_t* d_rows, size_t row_bytes, size_t n, uint8_t* d_codes, float4* d_meta, cudaStream_t stream);
 void launch_pq_decode(const float* d_codebook, size_t dims, size_t ncent, size_t nsub, const uint8_t* d_codes,
                       size_t code_stride, size_t n, float* d_vecs, cudaStream_t stream);
 // search.cu
@@ -198,11 +213,16 @@ struct SearchLaunch {
     uint32_t query_stride;
     uint32_t nq, k, L;
     uint32_t expand; // candidates expanded per round (1 = the reference's exact order)
+    bool screen;     // level-0 beam screens candidates with g.sq_codes before reading their rows (screen.cuh)
     uint64_t* out_keys;
     float* out_dists;
     uint32_t* out_counts;
 };
-uint32_t search_max_ctas(int dist_mode, int scalar_kind, const GraphView& g, uint32_t L, bool pq, uint32_t expand);
+uint32_t search_max_ctas(int dist_mode, int scalar_kind, const GraphView& g, uint32_t L, bool pq, uint32_t expand, bool screen);
+// test hook: screen bound and the search kernel's own fp32 distance for every (query, row) pair; device rows / queries
+// row_bytes apart, outputs [nq][n]
+void launch_screen_probe(int dist_mode, const uint8_t* d_rows, size_t n, const uint8_t* d_queries, size_t nq, uint32_t row_bytes,
+                         float* d_lb, float* d_dist, cudaStream_t stream);
 void launch_search(int dist_mode, int scalar_kind, bool pq, const SearchLaunch& p, cudaStream_t stream);
 // group.cu: the warp-per-query kernel as a single-GPU search path
 void launch_warp_search(Index& idx, const uint8_t* qbuf, size_t qrow, size_t nq, size_t k, uint32_t L, uint64_t* d_keys, float* d_dists,

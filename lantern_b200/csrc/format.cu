@@ -245,6 +245,7 @@ void Index::load_buffer(const void* buffer, size_t length) {
     LB_CUDA(cudaMemset(d_upper_adj_, 0xFF, upper_lists_cap_ * M * 4));
     if (n) {
         LB_CUDA(cudaMemcpy(d_vectors_, rows.data(), rows.size(), cudaMemcpyHostToDevice));
+        encode_screen(0, n);
         LB_CUDA(cudaMemcpy(d_adj0_, adj0.data(), adj0.size() * 4, cudaMemcpyHostToDevice));
         LB_CUDA(cudaMemcpy(d_upper_ref_, upper_ref.data(), upper_ref.size() * 4, cudaMemcpyHostToDevice));
         if (!upper_adj.empty())

@@ -19,6 +19,7 @@
 #include <cuda_runtime.h>
 #include <stdlib.h>
 
+#include <algorithm>
 #include <type_traits>
 
 #include "walk.cuh"
@@ -27,8 +28,7 @@ namespace lb200 {
 
 namespace {
 
-template <class W>
-__global__ void __launch_bounds__(kWalkThreads) hnsw_search_kernel(const __grid_constant__ SearchLaunch p, const uint32_t R) {
+template <class W> __device__ __forceinline__ void search_body(const SearchLaunch& p, const uint32_t R) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     const WalkLayout lay = W::layout(p.g, R, p.L, p.g.M0 * p.expand);
     W w(p.g);
@@ -73,11 +73,52 @@ __global__ void __launch_bounds__(kWalkThreads) hnsw_search_kernel(const __grid_
         atomicAdd(&p.s.counters[3], (unsigned long long)w.st_hops);
         if (w.st_limbo_drop)
             atomicAdd(&p.s.counters[4], (unsigned long long)w.st_limbo_drop);
+        if constexpr (W::kScreen) {
+            atomicAdd(&p.s.counters[5], (unsigned long long)sm.ctrl->screened);
+            atomicAdd(&p.s.counters[6], (unsigned long long)sm.ctrl->rejected);
+        }
+    }
+}
+
+template <class W>
+__global__ void __launch_bounds__(kWalkThreads) hnsw_search_kernel(const __grid_constant__ SearchLaunch p, const uint32_t R) {
+    search_body<W>(p, R);
+}
+// The screened walker (ScreenEval).  Up to NQ = 6 (d <= 768) it is capped at 64 registers, 8 CTAs/SM like the plain kernel: left to
+// itself the compiler takes 72 registers there, which costs the eighth resident CTA; capped, it spills a few words.
+template <class W>
+__global__ void __launch_bounds__(kWalkThreads, W::kMinCtas) hnsw_search_screen_kernel(const __grid_constant__ SearchLaunch p,
+                                                                                    const uint32_t R) {
+    search_body<W>(p, R);
+}
+template <class W> constexpr auto search_kernel_of() {
+    if constexpr (W::kScreen)
+        return hnsw_search_screen_kernel<W>;
+    else
+        return hnsw_search_kernel<W>;
+}
+
+// test hook (lb200_search_screen_probe): the screen's bound and row_distance() for every (query, row) pair, with the device
+// functions the search kernel uses.  One CTA per query, one warp per row.
+template <int DM, int NQ>
+__global__ void __launch_bounds__(128) screen_probe_kernel(const uint8_t* rows, uint32_t n, const uint8_t* queries, uint32_t row_bytes,
+                                                           const uint8_t* codes, const float4* meta, float* out_lb, float* out_d) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t nchunks = row_bytes / 16, cb = screen_code_bytes(row_bytes);
+    uint4 qreg[NQ];
+    const float a2 = load_qreg<DM, SK_F32, NQ>(qreg, queries + (size_t)blockIdx.x * row_bytes, nchunks, lane);
+    for (uint32_t j = warp; j < n; j += blockDim.x / 32) {
+        const float4 mt = meta[j];
+        const float s = screen_sum<DM, NQ>(qreg, reinterpret_cast<const uint32_t*>(codes + (size_t)j * cb), mt.x, nchunks, lane);
+        const float lb = screen_bound<DM, NQ>(s, mt, a2);
+        const float d = row_distance<DM, SK_F32, NQ>(qreg, reinterpret_cast<const uint4*>(rows + (size_t)j * row_bytes), nchunks, a2, lane);
+        if (lane == 0)
+            out_lb[(size_t)blockIdx.x * n + j] = lb, out_d[(size_t)blockIdx.x * n + j] = d;
     }
 }
 
 template <class W> void launch_one(const SearchLaunch& p, uint32_t R, size_t smem, uint32_t grid, int threads, cudaStream_t stream) {
-    auto kern = hnsw_search_kernel<W>;
+    auto kern = search_kernel_of<W>();
     LB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kern<<<grid, threads, smem, stream>>>(p, R);
     LB_CUDA(cudaGetLastError());
@@ -85,11 +126,21 @@ template <class W> void launch_one(const SearchLaunch& p, uint32_t R, size_t sme
 }
 
 template <class W> int occupancy_one(size_t smem, int threads) {
-    auto kern = hnsw_search_kernel<W>;
+    auto kern = search_kernel_of<W>();
     LB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int blocks = 0;
     LB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, threads, smem));
     return blocks;
+}
+
+// fn(walker type tag) with the screened walker of an f32 l2sq / cos index
+template <typename Fn> void dispatch_screen(int dm, int nq, Fn&& fn) {
+    dispatch_walk(dm, SK_F32, nq, [&](auto d, auto s, auto n) {
+        if constexpr (decltype(s)::value == SK_F32 && (decltype(d)::value == DM_L2SQ || decltype(d)::value == DM_COS))
+            fn(TypeTag<ScreenWalker<decltype(d)::value, decltype(n)::value>>{});
+        else
+            throw CudaError("search screen: f32 l2sq / cos indexes only");
+    });
 }
 
 } // namespace
@@ -111,7 +162,7 @@ static size_t search_smem(const GraphView& g, bool pq, uint32_t R, uint32_t L, u
               : walk_layout(R, g.row_bytes, L, g.M0 * expand).total;
 }
 
-uint32_t search_max_ctas(int dist_mode, int scalar_kind, const GraphView& g, uint32_t L, bool pq, uint32_t expand) {
+uint32_t search_max_ctas(int dist_mode, int scalar_kind, const GraphView& g, uint32_t L, bool pq, uint32_t expand, bool screen) {
     const uint32_t R = pick_ring_slots(g.row_bytes);
     const int nq = pq ? 1 : pick_nq(g.row_bytes);
     if (nq < 0)
@@ -119,7 +170,11 @@ uint32_t search_max_ctas(int dist_mode, int scalar_kind, const GraphView& g, uin
     const size_t smem = search_smem(g, pq, R, L, expand);
     int occ = 0;
     const int threads = search_threads(g, pq);
-    dispatch_walker(pq, dist_mode, scalar_kind, nq, [&](auto tag) { occ = occupancy_one<typename decltype(tag)::type>(smem, threads); });
+    auto occ_fn = [&](auto tag) { occ = occupancy_one<typename decltype(tag)::type>(smem, threads); };
+    if (screen)
+        dispatch_screen(dist_mode, nq, occ_fn);
+    else
+        dispatch_walker(pq, dist_mode, scalar_kind, nq, occ_fn);
     if (occ < 1)
         throw CudaError("search: kernel does not fit on an SM (ef/k or the pq table too large for shared memory)");
     return (uint32_t)occ * (uint32_t)device_sm_count();
@@ -131,8 +186,47 @@ void launch_search(int dist_mode, int scalar_kind, bool pq, const SearchLaunch& 
     const size_t smem = search_smem(p.g, pq, R, p.L, p.expand);
     const uint32_t grid = p.s.ctas < p.nq ? p.s.ctas : p.nq;
     const int threads = search_threads(p.g, pq);
-    dispatch_walker(pq, dist_mode, scalar_kind, nq,
-                    [&](auto tag) { launch_one<typename decltype(tag)::type>(p, R, smem, grid, threads, stream); });
+    auto launch_fn = [&](auto tag) { launch_one<typename decltype(tag)::type>(p, R, smem, grid, threads, stream); };
+    if (p.screen)
+        dispatch_screen(dist_mode, nq, launch_fn);
+    else
+        dispatch_walker(pq, dist_mode, scalar_kind, nq, launch_fn);
+}
+
+void launch_screen_probe(int dist_mode, const uint8_t* d_rows, size_t n, const uint8_t* d_queries, size_t nq, uint32_t row_bytes,
+                         float* d_lb, float* d_dist, cudaStream_t stream) {
+    const int nqr = pick_nq(row_bytes);
+    if (nqr < 0)
+        throw CudaError("screen probe: vectors wider than 8192 bytes are not supported");
+    const size_t cb = screen_code_bytes(row_bytes);
+    uint8_t* codes = nullptr;
+    float4* meta = nullptr;
+    LB_CUDA(cudaMalloc(&codes, std::max<size_t>(n * cb, 1)));
+    cudaError_t e = cudaMalloc(&meta, std::max<size_t>(n, 1) * sizeof(float4));
+    if (e != cudaSuccess) {
+        cudaFree(codes);
+        LB_CUDA(e);
+    }
+    try {
+        launch_sq_encode(d_rows, row_bytes, n, codes, meta, stream);
+        dispatch_walk(dist_mode, SK_F32, nqr, [&](auto d, auto s, auto q) {
+            constexpr int DM = decltype(d)::value;
+            if constexpr (decltype(s)::value == SK_F32 && (DM == DM_L2SQ || DM == DM_COS)) {
+                if (n && nq)
+                    screen_probe_kernel<DM, decltype(q)::value><<<(unsigned)nq, 128, 0, stream>>>(d_rows, (uint32_t)n, d_queries, row_bytes,
+                                                                                              codes, meta, d_lb, d_dist);
+                LB_CUDA(cudaGetLastError());
+                count_launch();
+            } else {
+                throw CudaError("screen probe: l2sq or cos only");
+            }
+        });
+        LB_CUDA(cudaStreamSynchronize(stream));
+    } catch (...) {
+        cudaFree(codes), cudaFree(meta);
+        throw;
+    }
+    cudaFree(codes), cudaFree(meta);
 }
 
 } // namespace lb200

@@ -22,6 +22,7 @@
 
 #include "distance.cuh"
 #include "engine.h"
+#include "screen.cuh"
 
 namespace lb200 {
 
@@ -35,6 +36,9 @@ struct WalkCtrl {
     uint32_t n;        // candidates in cand_id[], or kDone
     uint32_t ntouched; // entries in the touched list
     uint32_t top_size; // size of the top list after a beam
+    uint32_t m;        // screened walkers: candidates left after the screen
+    float radius;      // screened walkers: radius the round's candidates are screened against (NaN = no screen this round)
+    uint32_t screened, rejected; // screened walkers: candidates screened / rejected by this CTA (kept here, not in registers)
 };
 
 struct WalkSmem {
@@ -190,8 +194,41 @@ struct TopSmem { // arrays in shared memory
     __device__ __forceinline__ void flush(int) {}
 };
 
+// value -> registers (lane l holds chunks l, l+32, ...); returns |value|^2 for cos (0 otherwise)
+template <int DM, int SK, int NQ>
+__device__ __forceinline__ float load_qreg(uint4 (&qreg)[NQ], const uint8_t* row, uint32_t nchunks, int lane) {
+    const uint4* qg = reinterpret_cast<const uint4*>(row);
+    float part = 0.f;
+#pragma unroll
+    for (int i = 0; i < NQ; ++i) {
+        uint32_t c = lane + 32 * i;
+        qreg[i] = c < nchunks ? __ldg(qg + c) : make_uint4(0, 0, 0, 0);
+        part = norm_add(part, query_norm_chunk<DM, SK>(qreg[i]));
+    }
+    if constexpr (DM == DM_COS)
+        return warp_sum(part);
+    return 0.f;
+}
+
+// distance value (registers) -> one stored row (shared or global memory); every lane receives it
+template <int DM, int SK, int NQ>
+__device__ __forceinline__ float row_distance(const uint4 (&qreg)[NQ], const uint4* row, uint32_t nchunks, float a2, int lane) {
+    DistAcc<DM, SK> acc;
+    acc.reset();
+#pragma unroll
+    for (int i = 0; i < NQ; ++i) {
+        uint32_t c = lane + 32 * i;
+        if (c < nchunks) {
+            uint4 r = row[c];
+            accum_chunk<DM, SK>(acc, qreg[i], r);
+        }
+    }
+    return finish_distance<DM, SK>(acc, a2);
+}
+
 // state shared by every evaluator / walker
 struct WalkBase {
+    static constexpr bool kScreen = false; // ScreenEval: the level-0 beam screens candidates before measuring them
     const GraphView& g; // the kernel's own (__grid_constant__) parameter: fields are read from the constant bank
     WalkSmem sm;
     uint32_t* vis;
@@ -250,16 +287,9 @@ template <int DM, int SK, int NQ> struct RowEval : WalkBase {
 
     // value -> registers; every warp keeps its own copy.  `row` points to a 16-byte padded row in global memory.
     __device__ __forceinline__ void load_value(const uint8_t* row) {
-        const uint4* qg = reinterpret_cast<const uint4*>(row);
-        float part = 0.f;
-#pragma unroll
-        for (int i = 0; i < NQ; ++i) {
-            uint32_t c = lane + 32 * i;
-            qreg[i] = c < nchunks ? __ldg(qg + c) : make_uint4(0, 0, 0, 0);
-            part = norm_add(part, query_norm_chunk<DM, SK>(qreg[i]));
-        }
+        const float n2 = load_qreg<DM, SK, NQ>(qreg, row, nchunks, lane);
         if constexpr (DM == DM_COS)
-            a2 = warp_sum(part);
+            a2 = n2;
     }
     // a stored node becomes the value (refine_: candidate vs accepted; reverse links: target vs its neighbours)
     __device__ __forceinline__ void load_node(uint32_t id) { load_value(g.vectors + (size_t)id * g.row_bytes); }
@@ -271,19 +301,7 @@ template <int DM, int SK, int NQ> struct RowEval : WalkBase {
         bulk_g2s(sm.ring + (size_t)slot * g.row_bytes, g.vectors + (size_t)id * g.row_bytes, g.row_bytes, bar);
     }
 
-    __device__ __forceinline__ float row_distance(const uint4* row) const {
-        DistAcc<DM, SK> acc;
-        acc.reset();
-#pragma unroll
-        for (int i = 0; i < NQ; ++i) {
-            uint32_t c = lane + 32 * i;
-            if (c < nchunks) {
-                uint4 r = row[c];
-                accum_chunk<DM, SK>(acc, qreg[i], r);
-            }
-        }
-        return finish_distance<DM, SK>(acc, a2);
-    }
+    __device__ __forceinline__ float row_distance(const uint4* row) const { return lb200::row_distance<DM, SK, NQ>(qreg, row, nchunks, a2, lane); }
 
     // distances value -> cand_id[0..n) into cand_d[0..n).  Callers bracket it with __syncthreads().
     __device__ __forceinline__ void eval(uint32_t n) {
@@ -305,6 +323,87 @@ template <int DM, int SK, int NQ> struct RowEval : WalkBase {
             }
             si = (si + 1 == SPW) ? 0 : si + 1;
         }
+    }
+};
+
+// ---- f32 rows with the int8 screen (screen.cuh, DESIGN.md 4.1): the search kernel's evaluator for l2sq / cos -------------
+// screen(n, radius) runs between the compaction of a round's unseen candidates and eval(): every warp fetches the code rows
+// of its candidates (j % NW == warp) into its own ring slots with bulk copies, all issued before the first wait, computes
+// their bounds, and warp 0 keeps, in stored order, the candidates with !(lb >= radius).  Only those are measured; a rejected
+// one has d >= lb >= radius and the replay would have rejected it too, so the walk is unchanged.  eval() itself is untouched.
+template <int DM, int NQ> struct ScreenEval : RowEval<DM, SK_F32, NQ> {
+    using Base = RowEval<DM, SK_F32, NQ>;
+    static constexpr bool kScreen = true;
+    // search.cu: hnsw_search_screen_kernel's launch bounds = the CTAs/SM the plain kernel reaches with its own register count
+    static constexpr int kMinCtas = NQ <= 6 ? 8 : NQ <= 8 ? 7 : NQ <= 12 ? 5 : 4;
+
+    __device__ __forceinline__ explicit ScreenEval(const GraphView& gv) : Base(gv) {}
+    __device__ __forceinline__ void init(uint8_t* smem_raw, const WalkLayout& lay, uint32_t ring_slots, const SearchScratch& s) {
+        Base::init(smem_raw, lay, ring_slots, s);
+        if (threadIdx.x == 0)
+            this->sm.ctrl->screened = this->sm.ctrl->rejected = 0; // read back after the CTA's last barrier
+    }
+
+    // cand_id[0..n) -> its survivors, compacted in order; returns their number (uniform across the CTA)
+    __device__ __forceinline__ uint32_t screen(uint32_t n, float radius) {
+        const GraphView& g = this->g;
+        WalkSmem& sm = this->sm;
+        const int warp = this->warp, lane = this->lane;
+        const uint32_t NW = this->NW, rb = g.row_bytes, cb = screen_code_bytes(rb);
+        const uint32_t per_slot = rb / cb; // code rows per ring slot (>= 1; 4 at d = 768)
+        const uint32_t cap = min(this->SPW * per_slot, 32u);
+        const uint32_t T = n > (uint32_t)warp ? (n - warp + NW - 1) / NW : 0;
+        for (uint32_t t0 = 0; t0 < T; t0 += cap) {
+            const uint32_t cnt = min(cap, T - t0), nslots = (cnt + per_slot - 1) / per_slot;
+            fence_proxy_async(); // our generic-proxy reads of these slots (previous pass or round) precede the async writes
+            __syncwarp();
+            float4 meta = make_float4(0.f, 0.f, 0.f, 0.f);
+            if ((uint32_t)lane < nslots) {
+                const uint32_t slot = warp + NW * lane, k = min(per_slot, cnt - lane * per_slot);
+                uint64_t* bar = &sm.full[slot];
+                mbar_arrive_expect_tx(bar, k * cb);
+                for (uint32_t j = 0; j < k; ++j) {
+                    const uint32_t id = sm.cand_id[warp + NW * (t0 + lane * per_slot + j)];
+                    bulk_g2s(sm.ring + (size_t)slot * rb + j * cb, g.sq_codes + (size_t)id * cb, cb, bar);
+                }
+            }
+            if ((uint32_t)lane < cnt)
+                meta = __ldg(g.sq_meta + sm.cand_id[warp + NW * (t0 + lane)]);
+            float mine = 0.f;
+            for (uint32_t t = 0; t < cnt; ++t) {
+                const uint32_t si = t / per_slot, j = t - si * per_slot, slot = warp + NW * si;
+                if (j == 0) {
+                    mbar_wait(&sm.full[slot], (this->phase_bits >> si) & 1u);
+                    this->phase_bits ^= 1u << si;
+                }
+                const float scale = __shfl_sync(0xffffffffu, meta.x, t);
+                const float s = screen_sum<DM, NQ>(this->qreg, reinterpret_cast<const uint32_t*>(sm.ring + (size_t)slot * rb + j * cb),
+                                                   scale, this->nchunks, lane);
+                if ((uint32_t)lane == t)
+                    mine = s;
+            }
+            if ((uint32_t)lane < cnt)
+                sm.cand_d[warp + NW * (t0 + lane)] = screen_bound<DM, NQ>(mine, meta, this->a2);
+        }
+        fence_proxy_async(); // the code reads precede eval's bulk copies into the same slots
+        __syncthreads();
+        if (warp == 0) {
+            uint32_t m = 0;
+            for (uint32_t base = 0; base < n; base += 32) {
+                const uint32_t j = base + lane;
+                const bool keep = j < n && !(sm.cand_d[j] >= radius);
+                const uint32_t id = j < n ? sm.cand_id[j] : 0u;
+                const uint32_t mk = __ballot_sync(0xffffffffu, keep);
+                __syncwarp();
+                if (keep)
+                    sm.cand_id[m + __popc(mk & ((1u << lane) - 1u))] = id;
+                m += __popc(mk);
+            }
+            if (lane == 0)
+                sm.ctrl->m = m, sm.ctrl->screened += n, sm.ctrl->rejected += n - m;
+        }
+        __syncthreads();
+        return sm.ctrl->m;
     }
 };
 
@@ -674,17 +773,26 @@ template <class E> struct WalkerT : E {
                     }
                     st_pops += 1;
                 }
-                if (lane == 0)
+                if (lane == 0) {
                     sm.ctrl->n = popped ? n : kDone;
+                    if constexpr (E::kScreen) // the radius only shrinks within a round: screening against its start is safe
+                        sm.ctrl->radius = (level == 0 && top.size == L) ? top.radius(lane) : __int_as_float(0x7fffffff);
+                }
             }
             __syncthreads(); // (B)
-            const uint32_t n = sm.ctrl->n;
-            if (n == kDone)
+            const uint32_t n_all = sm.ctrl->n;
+            if (n_all == kDone)
                 break;
+            uint32_t n = n_all; // candidates measured (and replayed) this round
+            if constexpr (E::kScreen) {
+                const float r = sm.ctrl->radius;
+                if (r == r)
+                    n = this->screen(n_all, r);
+            }
             eval(n);
             __syncthreads(); // (C)
             if (warp == 0) {
-                st_dist += n;
+                st_dist += n_all; // the screen's rejects count as computed distances: the reference computes them
                 // index.hpp:3470 / :3382: accepted iff top.size() < top_limit || successor_dist < radius.  The radius only
                 // shrinks once the list is full, so a candidate that fails against the CURRENT radius can never pass
                 // later in this round: filter those out in parallel, then replay the survivors in stored order.
@@ -783,6 +891,7 @@ template <class E> struct WalkerT : E {
 
 template <int DM, int SK, int NQ> using Walker = WalkerT<RowEval<DM, SK, NQ>>;
 template <int DM> using PqWalker = WalkerT<PqEval<DM>>;
+template <int DM, int NQ> using ScreenWalker = WalkerT<ScreenEval<DM, NQ>>;
 
 // ---- (DM, SK, NQ) dispatch shared by the launchers ----------------------------------------------------
 // PQ indexes: fn(walker type tag) with PqWalker<DM>

@@ -1,0 +1,92 @@
+"""Dev experiment: the int8 search screen on vs off (LB200_SEARCH_SCREEN) on ONE built graph (needs a GPU).
+
+Builds a workload's graph once with bench.py's generator and seeds, then alternates the knob 0/1 for ROUNDS rounds of STEPS
+timed search steps each.  Prints, per setting, queries/s (median and spread over the rounds), kernel time, the share of
+candidates read in full (full_rows_read / computed_distances), that both settings return identical keys, distances and
+counters, and the device memory in use after the build and after the first search.
+usage: python scripts/exp_screen.py [workload] ; env ROUNDS (default 3), STEPS (default 20), OUT (directory for the JSON)"""
+import json, os, sys, time
+sys.path.insert(0, '.')
+import numpy as np, torch
+import bench
+from lantern_b200 import api
+
+wl_name = sys.argv[1] if len(sys.argv) > 1 else "cfg3"
+wl = bench.WORKLOADS[wl_name]
+rounds, steps = int(os.environ.get("ROUNDS", "3")), int(os.environ.get("STEPS", "20"))
+n, dim, B, k, ef = wl["n"], wl["dim"], wl["batch"], wl["k"], wl["ef"]
+dev = torch.device("cuda", 0)
+free0, total = torch.cuda.mem_get_info()
+X = bench.structured_torch(n, dim, bench.SEED_CORPUS, dev)
+pool = 4
+Q = bench.structured_torch(pool * B, dim, bench.SEED_QUERY, dev)
+idx = api.Index(dim, wl["metric"], "f32", M=wl["M"], efc=wl["efc"], ef=ef)
+idx.reserve(n)
+t = time.time()
+idx.add_batch_device(np.arange(1, n + 1, dtype=np.uint64), X.data_ptr(), n, dim * 4, "f32")
+idx.build()
+torch.cuda.synchronize()
+mem = {"total_gb": total / 1e9, "used_before_gb": (total - free0) / 1e9}
+mem["used_after_build_gb"] = (total - torch.cuda.mem_get_info()[0]) / 1e9
+print("%s: build %.1f s" % (wl_name, time.time() - t), flush=True)
+ok = torch.empty((B, k), dtype=torch.int64, device=dev)
+od = torch.empty((B, k), dtype=torch.float32, device=dev)
+oc = torch.empty((B,), dtype=torch.int32, device=dev)
+stream = torch.cuda.current_stream()
+
+
+def step(s):
+    idx.search_batch_device(Q[(s % pool) * B].data_ptr(), B, dim * 4, "f32", k, ef, ok.data_ptr(), od.data_ptr(), oc.data_ptr(),
+                            stream.cuda_stream)
+
+
+ref = {}
+for knob in ("0", "1"):  # outputs and counters of every pool batch, both ways
+    os.environ["LB200_SEARCH_SCREEN"] = knob
+    outs = []
+    t = time.time()
+    for s in range(pool):
+        step(s)
+        torch.cuda.synchronize()
+        st = idx.last_stats()
+        outs.append((ok.cpu().numpy().copy(), od.cpu().numpy().view(np.uint32).copy(), oc.cpu().numpy().copy(),
+                     st["computed_distances"], st["base_pops"], st["upper_hops"], st["full_rows_read"]))
+    ref[knob] = outs
+    print("screen=%s: %d checked batches in %.2f s" % (knob, pool, time.time() - t), flush=True)
+    if "used_after_search_gb" not in mem:
+        mem["used_after_search_gb"] = (total - torch.cuda.mem_get_info()[0]) / 1e9
+same = all(all(np.array_equal(a, b) for a, b in zip(o0[:3], o1[:3])) and o0[3:6] == o1[3:6] for o0, o1 in zip(ref["0"], ref["1"]))
+res = {"0": [], "1": []}
+kern = {"0": [], "1": []}
+for r in range(rounds):
+    for knob in ("0", "1"):
+        os.environ["LB200_SEARCH_SCREEN"] = knob
+        for s in range(3):
+            step(s)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        for s in range(steps):
+            step(s)
+        torch.cuda.synchronize()
+        res[knob].append(steps * B / (time.perf_counter() - t0))
+        km = 0.0
+        for s in range(4):
+            step(s)
+            km += idx.last_stats()["kernel_ms"]
+        kern[knob].append(km / 4)
+        print("round %d screen=%s  %.0f queries/s  kernel %.2f ms/step" % (r, knob, res[knob][-1], kern[knob][-1]), flush=True)
+out = {"workload": wl_name, "identical_outputs_and_counters": bool(same), "memory": mem,
+       "gpu": torch.cuda.get_device_name(0)}
+for knob in ("0", "1"):
+    v = np.array(res[knob])
+    cd = sum(o[3] for o in ref[knob])
+    fr = sum(o[6] for o in ref[knob])
+    out["screen_" + knob] = {"qps_median": float(np.median(v)), "qps_min": float(v.min()), "qps_max": float(v.max()),
+                             "kernel_ms_median": float(np.median(kern[knob])), "dist_evals_per_query": cd / (pool * B),
+                             "full_rows_read_per_query": fr / (pool * B), "full_rows_frac": fr / cd}
+out["speedup_median"] = out["screen_1"]["qps_median"] / out["screen_0"]["qps_median"]
+print(json.dumps(out))
+if os.environ.get("OUT"):  # directory for the JSON result
+    os.makedirs(os.environ["OUT"], exist_ok=True)
+    with open(os.path.join(os.environ["OUT"], "exp_screen_%s.json" % wl_name), "w") as f:
+        json.dump(out, f, indent=1)
