@@ -315,6 +315,14 @@ LB200_EXPORT void lb200_group_free(lb200_group_t, lb200_error_t* error);
 /* max_batch: largest nq of a search; max_results: largest nq * count (sizes the peer-mapped staging buffers). */
 LB200_EXPORT void lb200_group_distribute(lb200_group_t, lb200_index_t root_index, int root, size_t max_batch,
                                          size_t max_results, lb200_error_t* error);
+/* lb200_group_build: inserts every pending (and staged) vector of `root_index`, which lives on the device of rank `root`,
+ * with all ranks of a single-process group.  Every other rank works on a temporary replica of the index (freed when the call
+ * returns); each batch's new nodes are split between the ranks, and every list is written into every replica over NVLink.
+ * The result is what lb200_build gives on that index with the same batch cap: the same file, lb200_size and
+ * lb200_last_build_stats vectors and computed_distances.  `build_batch` still counts the nodes of a batch in total; its
+ * default (0) is the one-GPU default times the number of ranks.  The group's distribution is not touched: call
+ * lb200_group_distribute afterwards to search the new graph on the group.  Refused for multi-process groups. */
+LB200_EXPORT void lb200_group_build(lb200_group_t, lb200_index_t root_index, int root, lb200_error_t* error);
 /* host buffers in and out (host<->device copies included); counts may be NULL */
 LB200_EXPORT void lb200_group_search_batch(lb200_group_t, void const* queries, size_t nq, size_t stride,
                                            lb200_scalar_kind_t query_kind, size_t count, size_t ef, lb200_key_t* keys,

@@ -143,6 +143,7 @@ SIGNATURES = {
     "lb200_group_create_local": (C.c_void_p, [C.c_void_p, C.c_int, ERRP]),
     "lb200_group_free": (None, [C.c_void_p, ERRP]),
     "lb200_group_distribute": (None, [C.c_void_p, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, ERRP]),
+    "lb200_group_build": (None, [C.c_void_p, C.c_void_p, C.c_int, ERRP]),
     "lb200_group_search_batch": (None, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_size_t, C.c_size_t,
                                         C.c_void_p, C.c_void_p, C.c_void_p, ERRP]),
     "lb200_group_search_batch_device": (None, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_size_t, C.c_size_t,
@@ -376,6 +377,10 @@ class Group:
 
     def distribute(self, index, root=0, max_batch=8192, max_results=0):
         self._call("lb200_group_distribute", index.h if index is not None else None, root, max_batch, max_results)
+
+    def build(self, index, root=0):
+        """Insert every pending vector of `index` (on rank `root`'s device) with all ranks: lb200_build's graph, byte for byte."""
+        self._call("lb200_group_build", index.h if index is not None else None, root)
 
     def search_batch(self, queries, k, ef=0, nq=None, dim_bytes=None, kind=None):
         """Host buffers.  Non-root ranks of a multi-process group pass queries=None with nq / dim_bytes / kind."""

@@ -722,6 +722,9 @@ LB200_EXPORT void lb200_group_distribute(lb200_group_t h, lb200_index_t root_ind
                          max_results ? max_results : (max_batch ? max_batch : 8192) * 128);
     });
 }
+LB200_EXPORT void lb200_group_build(lb200_group_t h, lb200_index_t root_index, int root, lb200_error_t* error) {
+    guarded(error, [&] { group_build(*as_group(h), reinterpret_cast<Index*>(root_index), root); });
+}
 LB200_EXPORT void lb200_group_search_batch(lb200_group_t h, void const* queries, size_t nq, size_t stride,
                                            lb200_scalar_kind_t kind, size_t count, size_t ef, lb200_key_t* keys,
                                            lb200_distance_t* distances, size_t* counts, lb200_error_t* error) {

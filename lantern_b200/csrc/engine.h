@@ -257,6 +257,13 @@ void launch_merge_shards(const uint64_t* d_keys, const float* d_dists, size_t sh
                          uint64_t* d_out_keys, float* d_out_dists, cudaStream_t stream);
 // build.cu
 void build_pending(Index& idx);
+// the same build with every batch shared by the ranks of a single-process group (DESIGN.md 4.2): replicas[r] is rank r's
+// index and device, replicas[root].idx == &idx; the others are replicas of idx (group.cu) that receive every list it does
+struct BuildReplica {
+    Index* idx;
+    int device;
+};
+void build_pending_group(Index& idx, const std::vector<BuildReplica>& replicas, int root);
 // kmeans.cu
 int train_pq_codebook(const float* d_vectors, size_t stride_floats, size_t n, size_t dims, size_t nsub, size_t ncent, bool cosine,
                       size_t max_iter, uint64_t seed, const uint32_t* init_rows, float* d_codebook, cudaStream_t stream);

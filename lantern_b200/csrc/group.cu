@@ -30,6 +30,7 @@
 #include <algorithm>
 #include <chrono>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <vector>
 
@@ -1274,6 +1275,92 @@ void group_distribute(Group& G, Index* root_index, int root, size_t max_batch, s
     G.exchange(tick, all, 4); // nobody searches before everybody has mapped everybody
     G.root = root;
     G.distributed = true;
+}
+
+// A temporary copy of `root` on the current device for a group build: the root's config, codebook and PQ tables, its rows
+// [0, n0 + P), lists of nodes [0, n0), level-1+ lists and keys.  No search-screen companion: the build never reads it.
+static std::unique_ptr<Index> build_replica(Index& root) {
+    const IndexConfig& cfg = root.cfg_;
+    std::vector<float> codebook;
+    if (cfg.pq) {
+        codebook.resize(cfg.num_centroids * cfg.dims);
+        LB_CUDA(cudaMemcpy(codebook.data(), root.d_codebook_, codebook.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    }
+    std::unique_ptr<Index> x(new Index(cfg, codebook.data()));
+    x->sq_bytes_ = 0;
+    x->ensure_capacity(root.capacity_);
+    x->alloc_upper(root.upper_lists_);
+    const size_t n0 = root.n_, P = root.pending_n_;
+    auto copy = [](void* dst, const void* src, size_t bytes) {
+        if (bytes)
+            LB_CUDA(cudaMemcpy(dst, src, bytes, cudaMemcpyDefault));
+    };
+    copy(x->d_vectors_, root.d_vectors_, (n0 + P) * root.row_bytes_);
+    copy(x->d_adj0_, root.d_adj0_, n0 * cfg.M0 * sizeof(uint32_t));
+    copy(x->d_upper_ref_, root.d_upper_ref_, n0 * sizeof(uint32_t));
+    copy(x->d_upper_adj_, root.d_upper_adj_, root.upper_lists_ * cfg.M * sizeof(uint32_t));
+    copy(x->d_keys_, root.d_keys_, n0 * sizeof(uint64_t));
+    if (cfg.pq) { // the pair tables as the root computed them, and the raw pending rows (the value side of build distances)
+        copy(x->d_pq_pair_, root.d_pq_pair_, cfg.num_subvectors * cfg.num_centroids * cfg.num_centroids * sizeof(float));
+        copy(x->d_pq_norm_, root.d_pq_norm_, cfg.num_subvectors * cfg.num_centroids * sizeof(float));
+        const size_t raw = P * round_up(cfg.dims * 4, 16);
+        LB_CUDA(cudaMalloc(&x->d_pending_raw_, raw));
+        x->pending_raw_cap_ = raw;
+        copy(x->d_pending_raw_, root.d_pending_raw_, raw);
+        x->pq_max_code_ = root.pq_max_code_;
+    }
+    x->n_ = n0, x->upper_lists_ = root.upper_lists_, x->max_level_ = root.max_level_, x->entry_ = root.entry_;
+    LB_CUDA(cudaDeviceSynchronize());
+    return x;
+}
+
+void group_build(Group& G, Index* root_index, int root) {
+    DeviceGuard dg;
+    std::lock_guard<std::mutex> lk(G.mu);
+    // per-batch barriers between processes are not implemented: a world-1 group of lb200_group_create holds its only rank
+    if (G.ranks.size() != (size_t)G.world)
+        throw CudaError("group build: a multi-process group cannot build; create the group with lb200_group_create_local");
+    if (root < 0 || root >= G.world)
+        throw CudaError("group: bad root rank");
+    if (!root_index)
+        throw CudaError("null index handle");
+    Index& idx = *root_index;
+    const int dev = G.ranks[root]->device;
+    cudaPointerAttributes at;
+    LB_CUDA(cudaPointerGetAttributes(&at, idx.scratch_.counters));
+    if (at.device != dev)
+        throw CudaError("group build: the index does not live on the root rank's device");
+    LB_CUDA(cudaSetDevice(dev));
+    idx.flush_staged();
+    std::lock_guard<std::mutex> g(idx.mu_);
+    if (!idx.pending_n_)
+        return;
+    LB_CUDA(cudaDeviceSynchronize()); // the pending rows are written on the legacy stream
+    std::vector<std::unique_ptr<Index>> owned(G.world);
+    std::vector<BuildReplica> ranks(G.world);
+    try {
+        for (int r = 0; r < G.world; ++r) {
+            ranks[r].device = G.ranks[r]->device;
+            if (r == root) {
+                ranks[r].idx = &idx;
+                continue;
+            }
+            LB_CUDA(cudaSetDevice(ranks[r].device));
+            owned[r] = build_replica(idx);
+            ranks[r].idx = owned[r].get();
+        }
+        build_pending_group(idx, ranks, root);
+    } catch (...) {
+        for (int r = 0; r < G.world; ++r) {
+            cudaSetDevice(ranks[r].device);
+            owned[r].reset();
+        }
+        throw;
+    }
+    for (int r = 0; r < G.world; ++r) {
+        LB_CUDA(cudaSetDevice(ranks[r].device));
+        owned[r].reset();
+    }
 }
 
 // Message flags are (epoch mod 4096) << 20 | sequence number.  Before the 12-bit part wraps, every rank waits for its last

@@ -59,6 +59,7 @@ void group_free(Group* G);
 int group_world(const Group& G);
 int group_local_ranks(const Group& G);
 void group_distribute(Group& G, Index* root_index, int root, size_t max_batch, size_t max_results);
+void group_build(Group& G, Index* root_index, int root);
 void group_search_device(Group& G, const void* d_queries, size_t nq, size_t stride, int kind, size_t k, size_t ef,
                          uint64_t* d_keys, float* d_dists, uint32_t* d_counts, cudaStream_t stream);
 void group_search_host(Group& G, const void* queries, size_t nq, size_t stride, int kind, size_t k, size_t ef, uint64_t* keys,

@@ -14,8 +14,10 @@
 //   errors: <- u32 ERR_MSG 0x37333337, u32 length, text                            server.rs:563-573
 // The library underneath is the C ABI of include/lantern_b200.h; rows are handed to the GPU in blocks
 // (lb200_add_batch) instead of being fanned out over CPU threads (server.rs:317-359).  TLS and the router role
-// (server_type 2) are not implemented.
+// (server_type 2) are not implemented.  With --devices 0,1,... every session's index is built on a single-process group
+// of those GPUs (lb200_group_build, same file as the one-GPU build); the index lives on the first listed device.
 #include <arpa/inet.h>
+#include <dlfcn.h>
 #include <errno.h>
 #include <netinet/in.h>
 #include <netinet/tcp.h>
@@ -75,7 +77,27 @@ void check(lb200_error_t err) {
         throw std::runtime_error(err);
 }
 
-void serve(Conn& c, bool verbose) {
+// Makes `device` the current CUDA device of this thread through the driver API (the engine's runtime adopts the current
+// context), so that lb200_init allocates there.  Loaded at run time: without --devices the server needs no driver.
+bool make_device_current(int device) {
+    void* cu = dlopen("libcuda.so.1", RTLD_NOW);
+    if (!cu)
+        return false;
+    typedef int (*init_fn)(unsigned);
+    typedef int (*get_fn)(int*, int);
+    typedef int (*retain_fn)(void**, int);
+    typedef int (*set_fn)(void*);
+    init_fn cu_init = (init_fn)dlsym(cu, "cuInit");
+    get_fn cu_device_get = (get_fn)dlsym(cu, "cuDeviceGet");
+    retain_fn cu_retain = (retain_fn)dlsym(cu, "cuDevicePrimaryCtxRetain");
+    set_fn cu_set = (set_fn)dlsym(cu, "cuCtxSetCurrent");
+    int dev = 0;
+    void* ctx = nullptr;
+    return cu_init && cu_device_get && cu_retain && cu_set && cu_init(0) == 0 && cu_device_get(&dev, device) == 0 &&
+           cu_retain(&ctx, dev) == 0 && cu_set(ctx) == 0;
+}
+
+void serve(Conn& c, bool verbose, lb200_group_t group) {
     const uint32_t hello[2] = {kProtocolVersion, kServerType};
     c.write_all(hello, sizeof(hello));
 
@@ -174,7 +196,10 @@ void serve(Conn& c, bool verbose) {
             flush();
     }
     flush();
-    lb200_build(idx, &err);
+    if (group)
+        lb200_group_build(group, idx, 0, &err);
+    else
+        lb200_build(idx, &err);
     check(err);
 
     const uint64_t count = lb200_size(idx, &err);
@@ -200,6 +225,7 @@ int main(int argc, char** argv) {
     int port = 8998; // lantern_extras/src/lib.rs:172-237 hosts the reference server on 127.0.0.1:8998
     int max_sessions = -1;
     bool verbose = true;
+    std::vector<int> devices;
     for (int i = 1; i < argc; ++i) {
         std::string a = argv[i];
         if (a == "--host" && i + 1 < argc)
@@ -210,12 +236,35 @@ int main(int argc, char** argv) {
             max_sessions = atoi(argv[++i]);
         else if (a == "--quiet")
             verbose = false;
-        else {
-            fprintf(stderr, "usage: %s [--host H] [--port P] [--sessions N] [--quiet]\n", argv[0]);
+        else if (a == "--devices" && i + 1 < argc) { // e.g. 0,1,2,3: build every index on a group of these GPUs
+            const std::string list = argv[++i];
+            for (size_t at = 0; at < list.size();) {
+                devices.push_back(atoi(list.c_str() + at));
+                const size_t comma = list.find(',', at);
+                if (comma == std::string::npos)
+                    break;
+                at = comma + 1;
+            }
+        } else {
+            fprintf(stderr, "usage: %s [--host H] [--port P] [--sessions N] [--quiet] [--devices 0,1,...]\n", argv[0]);
             return 2;
         }
     }
     signal(SIGPIPE, SIG_IGN);
+    lb200_group_t group = nullptr;
+    if (!devices.empty()) {
+        if (!make_device_current(devices[0])) {
+            fprintf(stderr, "cannot make CUDA device %d current\n", devices[0]);
+            return 1;
+        }
+        lb200_error_t err = nullptr;
+        group = lb200_group_create_local(devices.data(), (int)devices.size(), &err);
+        if (err) {
+            fprintf(stderr, "lb200_group: %s\n", err);
+            return 1;
+        }
+        fprintf(stderr, "lb200_index_server: building on %zu GPUs (single-process group)\n", devices.size());
+    }
     int ls = socket(AF_INET, SOCK_STREAM, 0);
     if (ls < 0) {
         fprintf(stderr, "cannot create a socket: %s\n", strerror(errno));
@@ -249,7 +298,7 @@ int main(int argc, char** argv) {
         setsockopt(fd, SOL_SOCKET, SO_RCVTIMEO, &tv, sizeof(tv));
         Conn c{fd};
         try {
-            serve(c, verbose);
+            serve(c, verbose, group);
         } catch (const std::exception& e) { // server.rs:563-573
             std::string msg = e.what();
             if (verbose)
@@ -267,5 +316,9 @@ int main(int argc, char** argv) {
         close(fd);
     }
     close(ls);
+    if (group) {
+        lb200_error_t err = nullptr;
+        lb200_group_free(group, &err);
+    }
     return 0;
 }
