@@ -165,7 +165,9 @@ LB200_EXPORT void lb200_last_build_stats(lb200_index_t, lb200_build_stats_t* sta
  *   "build_ratio"  a batch never exceeds (nodes already in the graph) / build_ratio (default 64);
  *   "search_expand" candidates expanded per search round (default 1 = the reference's exact order; 2..8 = relaxed order:
  *                  fewer serial rounds, slightly more distance evaluations, identical results at ef >= N and recall within
- *                  the +-0.5 % window otherwise). */
+ *                  the +-0.5 % window otherwise);
+ *   "pq_query_tables" PQ search: 1 (default) = compute the batch's look-up tables in one launch when they take at most 1 GB,
+ *                  0 = never (each CTA builds its query's table, as it always does for larger batches; same results). */
 LB200_EXPORT void lb200_set_option(lb200_index_t, char const* name, size_t value, lb200_error_t* error);
 
 /* ---- search path: usearch.h:277-296, lib.cpp:389-410 ------------------------------------------ */
@@ -246,6 +248,15 @@ LB200_EXPORT void lb200_exact_tc_probe(float const* dataset, size_t dataset_size
 LB200_EXPORT void lb200_search_screen_probe(float const* dataset, size_t dataset_size, float const* queries, size_t queries_size,
                                             size_t dimensions, lb200_metric_kind_t metric_kind, float* lb, float* d,
                                             lb200_error_t* error);
+/* Test hook, not a search entry point: the asymmetric distances of a built PQ index, computed by the evaluator the search and
+ * build kernels use.  mode 0: `count` raw f32 values (values[count][dimensions]) with the look-up tables a search batch
+ * precomputes; mode 1: the same values with the tables each CTA builds itself (batches past 1 GB, and the build); mode 2:
+ * stored nodes nodes[count] as values, tables from the centroid-pair table (refine and reverse links).  rows / lut_width
+ * (may be NULL) receive the stored rows n and the table width W; with distances == NULL nothing runs.  Outputs
+ * distances[count][n] (value against every stored row) and tables[count][num_subvectors * W + 1] (the table, then |value|^2,
+ * 0 for l2sq values built in the kernel, which do not use it); host memory. */
+LB200_EXPORT void lb200_pq_probe(lb200_index_t, int mode, float const* values, uint32_t const* nodes, size_t count, size_t* rows,
+                                 size_t* lut_width, float* distances, float* tables, lb200_error_t* error);
 /* f32 -> f16 / i8 / b1 (index_plugins.hpp:879-974); host memory; `count` vectors. */
 LB200_EXPORT void lb200_cast(lb200_scalar_kind_t from, void const* vectors, lb200_scalar_kind_t to, void* result,
                              size_t result_size, int dims, lb200_error_t* error);

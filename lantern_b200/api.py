@@ -127,6 +127,8 @@ SIGNATURES = {
                                     C.c_void_p, C.c_void_p, C.c_void_p, ERRP]),
     "lb200_search_screen_probe": (None, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_void_p,
                                          C.c_void_p, ERRP]),
+    "lb200_pq_probe": (None, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t),
+                              C.POINTER(C.c_size_t), C.c_void_p, C.c_void_p, ERRP]),
     "lb200_cast": (None, [C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_int, ERRP]),
     "lb200_cast_batch": (None, [C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_void_p, ERRP]),
     "lb200_quantize_pq": (None, [C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
@@ -198,6 +200,7 @@ class Index:
                  num_subvectors=0, codebook=None):
         L = lib()
         self.dim, self.metric, self.quant, self.M = dim, metric, quant, M
+        self.num_subvectors = num_subvectors
         o = InitOptions()
         o.metric_kind, o.quantization, o.dimensions = METRIC[metric], SCALAR[quant], dim
         o.connectivity, o.expansion_add, o.expansion_search = M, efc, ef
@@ -479,6 +482,29 @@ def search_screen_probe(dataset, queries, metric="l2sq"):
     d = np.zeros((len(Q), len(X)), np.float32)
     _static("lb200_search_screen_probe", _ptr(X), len(X), _ptr(Q), len(Q), X.shape[1], METRIC[metric], _ptr(lb), _ptr(d))
     return lb, d
+
+
+PQ_PROBE_MODES = {"batch": 0, "kernel": 1, "node": 2}
+
+
+def pq_probe(index, mode, values=None, nodes=None):
+    """Test hook on a built PQ index: (d [count][n], lut [count][nsub][W], v2 [count]) -- the search / build evaluator's
+    distance from each value to every stored row, the look-up table it used and |value|^2.  mode "batch" / "kernel": f32
+    values with the batch's precomputed tables / tables built in the kernel; "node": stored node ids as values."""
+    m = PQ_PROBE_MODES[mode]
+    if m == 2:
+        vals, nd = None, np.ascontiguousarray(nodes, dtype=np.uint32)
+        count = len(nd)
+    else:
+        vals, nd = np.ascontiguousarray(values, dtype=np.float32), None
+        count = len(vals)
+    rows, width = C.c_size_t(), C.c_size_t()
+    index._call("lb200_pq_probe", m, _ptr(vals), _ptr(nd), count, C.byref(rows), C.byref(width), None, None)
+    n, W = rows.value, width.value
+    d = np.zeros((count, n), np.float32)
+    tab = np.zeros((count, index.num_subvectors * W + 1), np.float32)
+    index._call("lb200_pq_probe", m, _ptr(vals), _ptr(nd), count, None, None, _ptr(d), _ptr(tab))
+    return d, tab[:, :-1].reshape(count, index.num_subvectors, W), tab[:, -1].copy()
 
 
 def cast(vectors_f32, quant):

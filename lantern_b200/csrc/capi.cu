@@ -242,7 +242,9 @@ LB200_EXPORT void lb200_set_option(lb200_index_t h, char const* name, size_t val
             if (value > 2)
                 throw CudaError("search_kernel: 0, 1 or 2");
             idx->search_kernel_ = value;
-        } else if (n == "touched_cap") // testing knob: size of the per-CTA un-visit log
+        } else if (n == "pq_query_tables") // 1 = precompute a pq search batch's look-up tables when they fit in 1 GB, 0 = never
+            idx->pq_query_tables_ = value != 0;
+        else if (n == "touched_cap") // testing knob: size of the per-CTA un-visit log
             idx->touched_cap_ = (uint32_t)std::max<size_t>(value, 32);
         else
             throw CudaError("unknown option");
@@ -581,6 +583,53 @@ LB200_EXPORT void lb200_search_screen_probe(float const* dataset, size_t dataset
         launch_screen_probe(dm, dd.as<uint8_t>(), dataset_size, dq.as<uint8_t>(), queries_size, (uint32_t)rb, dl.as<float>(), dv.as<float>(), 0);
         LB_CUDA(cudaMemcpy(lb, dl.p, queries_size * dataset_size * 4, cudaMemcpyDeviceToHost));
         LB_CUDA(cudaMemcpy(d, dv.p, queries_size * dataset_size * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+LB200_EXPORT void lb200_pq_probe(lb200_index_t h, int mode, float const* values, uint32_t const* nodes, size_t count, size_t* rows,
+                                 size_t* lut_width, float* distances, float* tables, lb200_error_t* error) {
+    guarded(error, [&] {
+        Index* idx = as_index(h);
+        const IndexConfig& c = idx->config();
+        if (!c.pq)
+            throw CudaError("pq_probe: not a pq index");
+        if (mode < 0 || mode > 2)
+            throw CudaError("pq_probe: mode 0 (batch tables), 1 (tables built in the kernel) or 2 (node tables)");
+        idx->flush_staged();
+        std::lock_guard<std::mutex> g(idx->mu_);
+        if (idx->pending_n_)
+            throw CudaError("pq_probe: the index has vectors that are not built yet");
+        GraphView gv = idx->view();
+        if (rows)
+            *rows = gv.n;
+        if (lut_width)
+            *lut_width = gv.pq_lut_width;
+        if (!distances || !count || !gv.n)
+            return;
+        if (!tables || (mode == 2 ? !nodes : !values))
+            throw CudaError("pq_probe: null input or output buffer");
+        if (mode == 2)
+            for (size_t i = 0; i < count; ++i)
+                if (nodes[i] >= gv.n)
+                    throw CudaError("pq_probe: node id out of range");
+        const size_t vrow = round_up(c.dims * 4, 16), tf = (size_t)c.num_subvectors * gv.pq_lut_width;
+        DeviceTemp dv(mode == 2 ? count * 4 : count * vrow), dd(count * gv.n * 4), dl(count * (tf + 1) * 4),
+            dt(mode == 0 ? count * pq_table_floats((uint32_t)c.num_subvectors, gv.pq_lut_width) * 4 : 0);
+        if (mode == 2)
+            LB_CUDA(cudaMemcpy(dv.p, nodes, count * 4, cudaMemcpyHostToDevice));
+        else
+            upload_rows(values, count, c.dims * 4, SK_F32, c.dims, dv.as<uint8_t>(), vrow);
+        if (mode == 0) {
+            launch_pq_query_tables(idx->d_codebook_, c.dims, c.num_subvectors, gv.pq_lut_width, idx->dist_mode_ == DM_COS, dv.as<float>(),
+                                   vrow / 4, count, dt.as<float>(), 0);
+            gv.pq_query_tables = dt.as<float>();
+        }
+        // the search kernel's candidate capacity for this index
+        const uint32_t cand_cap = (uint32_t)(c.M0 * std::min<size_t>(std::max<size_t>(idx->search_expand_, 1), 8));
+        launch_pq_probe(idx->dist_mode_, gv, cand_cap, mode == 2 ? nullptr : dv.as<uint8_t>(), (uint32_t)vrow,
+                        mode == 2 ? dv.as<uint32_t>() : nullptr, count, dd.as<float>(), dl.as<float>(), 0);
+        LB_CUDA(cudaMemcpy(distances, dd.p, count * gv.n * 4, cudaMemcpyDeviceToHost));
+        LB_CUDA(cudaMemcpy(tables, dl.p, count * (tf + 1) * 4, cudaMemcpyDeviceToHost));
     });
 }
 

@@ -278,7 +278,7 @@ void launch_pq_query_tables(const float* d_codebook, size_t dims, size_t nsub, s
                             size_t q_stride_floats, size_t nq, float* d_tables, cudaStream_t stream) {
     if (!nq)
         return;
-    const size_t table_floats = nsub * lut_width + 4;
+    const size_t table_floats = pq_table_floats((uint32_t)nsub, (uint32_t)lut_width);
     pq_query_tables_kernel<<<(unsigned)nq, 256, dims * sizeof(float), stream>>>(d_codebook, (uint32_t)dims, (uint32_t)nsub,
                                                                                 (uint32_t)lut_width, cosine ? 1 : 0, d_queries,
                                                                                 q_stride_floats, d_tables, table_floats);

@@ -12,6 +12,7 @@
 
 #include "distance.cuh"
 #include "screen.cuh"
+#include "walk.cuh"
 
 namespace lb200 {
 
@@ -295,15 +296,28 @@ GraphView Index::view() const {
     g.dims = (uint32_t)cfg_.dims;
     g.num_centroids = (uint32_t)cfg_.num_centroids;
     g.num_subvectors = (uint32_t)cfg_.num_subvectors;
-    // the reference's encoder never emits centroid ids >= 128 (signed-char loop, lantern_storage.hpp:123) and neither does
-    // lb200_add*: then half of a 256-entry table can never be addressed and is not built (half the shared memory)
-    g.pq_lut_width = (uint32_t)((cfg_.num_centroids > 128 && pq_max_code_ < 128) ? 128 : cfg_.num_centroids);
+    g.pq_lut_width = pq_lut_width(cfg_.num_centroids, pq_max_code_);
     g.sq_codes = d_sq_codes_;
     g.sq_meta = d_sq_meta_;
     g.flags = 2u; // L2-prefetch the adjacency line of nodes that enter the top list
     if (const char* e = getenv("LB200_FLAGS"))
         g.flags = (uint32_t)atoi(e);
     return g;
+}
+
+// Sized for the walks that stage the value in the CTA and build its table there -- every build kernel, and the search of a
+// batch whose tables pass 1 GB -- with a top list of one and the level-0 candidates; larger ef or efc only add to it.  A
+// search with precomputed tables needs `dims` floats less, so a table that fits only that way could still answer small
+// batches, but could never be built on, inserted into or searched in large batches: such a file is refused too.
+void Index::check_pq_table_fits(uint32_t lut_width) const {
+    const size_t need = walk_layout_pq((uint32_t)cfg_.num_subvectors, lut_width, (uint32_t)cfg_.dims, 1, (uint32_t)cfg_.M0).total;
+    int dev = 0, limit = 0;
+    LB_CUDA(cudaGetDevice(&dev));
+    LB_CUDA(cudaDeviceGetAttribute(&limit, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    if (need > (size_t)limit)
+        throw CudaError("pq: the " + std::to_string(cfg_.num_subvectors) + " x " + std::to_string(lut_width) +
+                        " look-up table needs " + std::to_string(need) + " bytes of shared memory per CTA; the device allows " +
+                        std::to_string(limit));
 }
 
 void Index::ensure_scratch(uint32_t ctas) {
@@ -367,8 +381,8 @@ void Index::search_device(const void* d_queries, size_t nq, size_t stride, int k
     if (cfg_.pq) {
         // the batch's look-up tables in one dense launch (49 KB per query at 96 x 128): the walk kernel then fetches a table with
         // one bulk copy instead of computing nsub * ncent * subdim flops per query at 4 CTAs per SM
-        const size_t tbytes = nq * (cfg_.num_subvectors * (size_t)gv.pq_lut_width + 4) * sizeof(float);
-        if (tbytes <= ((size_t)1 << 30)) {
+        const size_t tbytes = nq * pq_table_floats((uint32_t)cfg_.num_subvectors, gv.pq_lut_width) * sizeof(float);
+        if (pq_query_tables_ && tbytes <= ((size_t)1 << 30)) {
             if (tbytes > pq_tables_bytes_) {
                 if (d_pq_tables_)
                     LB_CUDA(cudaFree(d_pq_tables_));

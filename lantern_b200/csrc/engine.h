@@ -66,6 +66,17 @@ struct GraphView {
     const float4* sq_meta;
 };
 
+// Floats of one value's PQ look-up table: [nsub][lut_width] padded to whole 16-byte chunks, then |value|^2 and 3 spare floats.
+// Precomputed tables travel to shared memory by bulk copy, whose size and addresses must be multiples of 16 bytes.
+LB_HD inline size_t pq_table_floats(uint32_t nsub, uint32_t lut_width) { return (nsub * lut_width + 7u) & ~3u; }
+
+// Centroids a PQ look-up table covers.  The reference's encoder never emits centroid ids >= 128 (signed-char loop,
+// lantern_storage.hpp:123) and neither does lb200_add*: then half of a 256-entry table can never be addressed and is not
+// built (half the shared memory).  A loaded file whose codes reach 128 needs every centroid.
+inline uint32_t pq_lut_width(size_t num_centroids, uint32_t max_code) {
+    return (uint32_t)((num_centroids > 128 && max_code < 128) ? 128 : num_centroids);
+}
+
 struct SearchScratch {
     uint32_t* visited;     // [ctas][words_per_cta]
     uint32_t* touched;     // [ctas][touched_cap]
@@ -130,6 +141,7 @@ class Index {
     uint32_t touched_cap_ = 16384; // per-CTA log of bitmap words to un-visit; beyond it the whole bitmap is cleared
     size_t search_expand_ = 1;  // 1 = exact-order search; 2..4 = relaxed order (see walk.cuh)
     size_t search_kernel_ = 0;  // 0 = pick by row width, 1 = one CTA per query (search.cu), 2 = one warp per query (group.cu)
+    bool pq_query_tables_ = true; // pq search: precompute the batch's look-up tables when they fit in 1 GB; false = never
     uint8_t* d_warp_aux_ = nullptr; // warp kernel: counters, flags, dummy counts
     size_t warp_aux_bytes_ = 0;
     double last_build_ms_ = 0;
@@ -184,6 +196,8 @@ class Index {
     std::mutex stream_mu_;
 
     void ensure_scratch(uint32_t ctas);
+    // throws unless a PQ walk with a look-up table `lut_width` centroids wide fits in one CTA's shared memory
+    void check_pq_table_fits(uint32_t lut_width) const;
     void encode_screen(size_t first, size_t count); // companion of rows [first, first + count) from d_vectors_
     void* io_buffer(size_t bytes);
     uint8_t* query_buffer(size_t bytes);
@@ -198,7 +212,7 @@ void launch_pq_encode(const float* d_codebook, size_t dims, size_t ncent, size_t
                       cudaStream_t stream);
 void launch_pq_tables(const float* d_codebook, size_t dims, size_t ncent, size_t nsub, bool cosine, float* d_pair, float* d_norm,
                       cudaStream_t stream);
-// per-query ADC tables of a batch: out[q][s * lut_width + c] (+ |q|^2 at [nsub * lut_width]), row stride = nsub*lut_width + 4 floats
+// per-query ADC tables of a batch: out[q][s * lut_width + c] (+ |q|^2 at [nsub * lut_width]), row stride pq_table_floats()
 void launch_pq_query_tables(const float* d_codebook, size_t dims, size_t nsub, size_t lut_width, bool cosine, const float* d_queries,
                             size_t q_stride_floats, size_t nq, float* d_tables, cudaStream_t stream);
 // screen.cuh companion of n stored f32 rows (row_bytes apart): codes[n][screen_code_bytes(row_bytes)], meta[n]
@@ -224,6 +238,11 @@ uint32_t search_max_ctas(int dist_mode, int scalar_kind, const GraphView& g, uin
 void launch_screen_probe(int dist_mode, const uint8_t* d_rows, size_t n, const uint8_t* d_queries, size_t nq, uint32_t row_bytes,
                          float* d_lb, float* d_dist, cudaStream_t stream);
 void launch_search(int dist_mode, int scalar_kind, bool pq, const SearchLaunch& p, cudaStream_t stream);
+// test hook: PqEval on the view `g` of a PQ index, for `count` values -- raw f32 rows value_stride bytes apart (tables from
+// g.pq_query_tables when set, else built in the kernel), or stored nodes when d_nodes != NULL.  Outputs d_dist[count][g.n]
+// (every stored row, measured cand_cap at a time) and d_lut[count][nsub * pq_lut_width + 1] (the table, then |value|^2).
+void launch_pq_probe(int dist_mode, const GraphView& g, uint32_t cand_cap, const uint8_t* d_values, uint32_t value_stride,
+                     const uint32_t* d_nodes, size_t count, float* d_dist, float* d_lut, cudaStream_t stream);
 // group.cu: the warp-per-query kernel as a single-GPU search path
 void launch_warp_search(Index& idx, const uint8_t* qbuf, size_t qrow, size_t nq, size_t k, uint32_t L, uint64_t* d_keys, float* d_dists,
                         uint32_t* d_counts, cudaStream_t stream);

@@ -231,6 +231,7 @@ void Index::load_buffer(const void* buffer, size_t length) {
                     throw CudaError("corrupted centroid id"); // lantern_storage.hpp:141
                 pq_max_code = std::max<uint32_t>(pq_max_code, c);
             }
+        check_pq_table_fits(pq_lut_width(cfg_.num_centroids, pq_max_code));
     }
     // commit (nothing below throws for a reason that depends on the file contents)
     pq_max_code_ = pq_max_code;

@@ -117,6 +117,50 @@ __global__ void __launch_bounds__(128) screen_probe_kernel(const uint8_t* rows, 
     }
 }
 
+// test hook (lb200_pq_probe): the walkers' own PqEval<DM> on the index's view.  CTA v turns value v into its look-up table
+// (load_query: the batch's precomputed tables when g.pq_query_tables is set, else load_value; load_node for node values),
+// copies the table and |v|^2 out, then measures every stored row through eval(), cand_cap rows per pass, as a walk does.
+template <int DM>
+__global__ void __launch_bounds__(kWalkThreads) pq_probe_kernel(const __grid_constant__ GraphView g, const uint8_t* values,
+                                                                uint32_t value_stride, const uint32_t* nodes, uint32_t cand_cap,
+                                                                float* out_d, float* out_lut) {
+    extern __shared__ __align__(128) uint8_t smem_raw[];
+    const WalkLayout lay = PqEval<DM>::layout(g, 0, 1, cand_cap);
+    PqEval<DM> w(g);
+    w.init(smem_raw, lay, 0, SearchScratch{});
+    const uint32_t v = blockIdx.x;
+    if (nodes)
+        w.load_node(nodes[v]);
+    else
+        w.load_query(v, values + (size_t)v * value_stride);
+    const size_t tf = (size_t)g.num_subvectors * g.pq_lut_width;
+    for (size_t e = threadIdx.x; e < tf; e += kWalkThreads)
+        out_lut[v * (tf + 1) + e] = w.lut[e];
+    if (threadIdx.x == 0)
+        out_lut[v * (tf + 1) + tf] = w.a2;
+    for (uint32_t base = 0; base < g.n; base += cand_cap) {
+        const uint32_t cnt = min(cand_cap, g.n - base);
+        __syncthreads();
+        for (uint32_t j = threadIdx.x; j < cnt; j += kWalkThreads)
+            w.sm.cand_id[j] = base + j;
+        __syncthreads();
+        w.eval(cnt);
+        __syncthreads();
+        for (uint32_t j = threadIdx.x; j < cnt; j += kWalkThreads)
+            out_d[(size_t)v * g.n + base + j] = w.sm.cand_d[j];
+    }
+}
+
+template <int DM>
+void launch_pq_probe_dm(const GraphView& g, uint32_t cand_cap, const uint8_t* d_values, uint32_t value_stride, const uint32_t* d_nodes,
+                        size_t count, float* d_dist, float* d_lut, cudaStream_t stream) {
+    const size_t smem = PqEval<DM>::layout(g, 0, 1, cand_cap).total;
+    LB_CUDA(cudaFuncSetAttribute(pq_probe_kernel<DM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    pq_probe_kernel<DM><<<(unsigned)count, kWalkThreads, smem, stream>>>(g, d_values, value_stride, d_nodes, cand_cap, d_dist, d_lut);
+    LB_CUDA(cudaGetLastError());
+    count_launch();
+}
+
 template <class W> void launch_one(const SearchLaunch& p, uint32_t R, size_t smem, uint32_t grid, int threads, cudaStream_t stream) {
     auto kern = search_kernel_of<W>();
     LB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -227,6 +271,19 @@ void launch_screen_probe(int dist_mode, const uint8_t* d_rows, size_t n, const u
         throw;
     }
     cudaFree(codes), cudaFree(meta);
+}
+
+void launch_pq_probe(int dist_mode, const GraphView& g, uint32_t cand_cap, const uint8_t* d_values, uint32_t value_stride,
+                     const uint32_t* d_nodes, size_t count, float* d_dist, float* d_lut, cudaStream_t stream) {
+    if (!count || !g.n)
+        return;
+    if (dist_mode == DM_L2SQ)
+        launch_pq_probe_dm<DM_L2SQ>(g, cand_cap, d_values, value_stride, d_nodes, count, d_dist, d_lut, stream);
+    else if (dist_mode == DM_COS)
+        launch_pq_probe_dm<DM_COS>(g, cand_cap, d_values, value_stride, d_nodes, count, d_dist, d_lut, stream);
+    else
+        throw CudaError("pq probe: l2sq or cos only");
+    LB_CUDA(cudaStreamSynchronize(stream));
 }
 
 } // namespace lb200

@@ -77,10 +77,10 @@ __host__ __device__ inline WalkLayout walk_layout_bytes(size_t stage_bytes, uint
 __host__ __device__ inline WalkLayout walk_layout(uint32_t R, uint32_t row_bytes, uint32_t top_cap, uint32_t cand_cap) {
     return walk_layout_bytes((size_t)R * row_bytes, R, top_cap, cand_cap);
 }
-// PQ: look-up table [nsub][ncent] (+ 4 floats: the value's squared norm travels with a precomputed table) + value staging
-// [dims] + per-warp partial sums [warps][2][64]; one mbarrier (bulk copy of a precomputed table)
+// PQ: look-up table of pq_table_floats(nsub, lut_width) floats ([nsub][lut_width] padded to whole 16-byte chunks, then the
+// value's squared norm, which travels with a precomputed table) + value staging [dims] + per-warp partial sums [warps][2][64];
+// one mbarrier (bulk copy of a precomputed table)
 constexpr uint32_t kPqPartPerWarp = 64;
-__host__ __device__ inline size_t pq_table_floats(uint32_t nsub, uint32_t lut_width) { return (size_t)nsub * lut_width + 4; }
 // `value_floats` = dims when the kernel builds tables itself from raw vectors (build; search without precomputed tables), else 0
 __host__ __device__ inline WalkLayout walk_layout_pq(uint32_t nsub, uint32_t lut_width, uint32_t value_floats, uint32_t top_cap, uint32_t cand_cap) {
     return walk_layout_bytes((pq_table_floats(nsub, lut_width) + value_floats + (size_t)kWalkWarps * 2 * kPqPartPerWarp) * 4, 1, top_cap, cand_cap);
