@@ -108,13 +108,16 @@ typedef struct lb200_search_stats_t {
     uint64_t computed_distances; /* == usearch search_result_t::computed_distances summed over the batch */
     uint64_t base_pops;          /* level-0 candidates expanded */
     uint64_t upper_hops;         /* level>=1 neighbour lists scanned */
-    uint64_t algorithmic_bytes;  /* full_rows_read*row_bytes + screened candidates*(code row + 16) + (base_pops*(4+4*M0) +
+    uint64_t algorithmic_bytes;  /* full_rows_read*row_bytes + screened candidates*(code row + 16, or the projected record) +
+                                    (base_pops*(4+4*M0) +
                                     upper_hops*(4+4*M)) + queries*row_bytes: the bytes the search needed */
     double kernel_ms;            /* device time of the search kernel alone (CUDA events on the launching stream) */
     uint64_t limbo_overflows;    /* equal-distance candidates beyond the 64 the walker parks at the eviction boundary (only
                                     possible with massive exact ties; each one may be an expansion the reference performs) */
     uint64_t full_rows_read;     /* (appended field) stored rows read in full: computed_distances minus the candidates the
-                                    int8 screen of f32 l2sq / cos searches rejected from their codes alone */
+                                    screen of f32 l2sq / cos searches rejected from their codes alone */
+    uint32_t screen_kind;        /* (appended field) the search's screen: 0 none, 1 int8 codes of every dimension, 2 projected codes */
+    uint32_t screen_dims;        /* (appended field) codes per screened candidate: dimensions (1) or the basis' k (2) */
 } lb200_search_stats_t;
 
 /* Work of the most recent lb200_build (or implicit build): the build metric of SURVEY.md 8d is
@@ -248,6 +251,14 @@ LB200_EXPORT void lb200_exact_tc_probe(float const* dataset, size_t dataset_size
 LB200_EXPORT void lb200_search_screen_probe(float const* dataset, size_t dataset_size, float const* queries, size_t queries_size,
                                             size_t dimensions, lb200_metric_kind_t metric_kind, float* lb, float* d,
                                             lb200_error_t* error);
+/* Test hook, like lb200_search_screen_probe, for the projected screen: `basis` = k x dimensions fp32 (any values), or NULL for
+ * the rows' own basis (the top-k eigenvectors of their second moment; k = 0: chosen as an index chooses it, or its best k). */
+LB200_EXPORT void lb200_search_pscreen_probe(float const* dataset, size_t dataset_size, float const* queries, size_t queries_size,
+                                             size_t dimensions, lb200_metric_kind_t metric_kind, float const* basis, size_t k, float* lb,
+                                             float* d, lb200_error_t* error);
+/* The projected screen's basis of an index: returns k (0 = the index keeps none) and, when `basis` is not NULL, copies the
+ * k x dimensions fp32 basis there; `seconds` (may be NULL) receives the host time its last choice took. */
+LB200_EXPORT size_t lb200_screen_basis(lb200_index_t, float* basis, double* seconds, lb200_error_t* error);
 /* Test hook, not a search entry point: the asymmetric distances of a built PQ index, computed by the evaluator the search and
  * build kernels use.  mode 0: `count` raw f32 values (values[count][dimensions]) with the look-up tables a search batch
  * precomputes; mode 1: the same values with the tables each CTA builds itself (batches past 1 GB, and the build); mode 2:

@@ -55,7 +55,8 @@ class IndexMetadata(C.Structure):  # == usearch_index_metadata_t (usearch.h:119-
 class SearchStats(C.Structure):
     _fields_ = [("queries", C.c_uint64), ("computed_distances", C.c_uint64), ("base_pops", C.c_uint64),
                 ("upper_hops", C.c_uint64), ("algorithmic_bytes", C.c_uint64), ("kernel_ms", C.c_double),
-                ("limbo_overflows", C.c_uint64), ("full_rows_read", C.c_uint64)]
+                ("limbo_overflows", C.c_uint64), ("full_rows_read", C.c_uint64), ("screen_kind", C.c_uint32),
+                ("screen_dims", C.c_uint32)]
 
 
 class BuildStats(C.Structure):
@@ -127,6 +128,9 @@ SIGNATURES = {
                                     C.c_void_p, C.c_void_p, C.c_void_p, ERRP]),
     "lb200_search_screen_probe": (None, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_void_p,
                                          C.c_void_p, ERRP]),
+    "lb200_search_pscreen_probe": (None, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_void_p,
+                                          C.c_size_t, C.c_void_p, C.c_void_p, ERRP]),
+    "lb200_screen_basis": (C.c_size_t, [C.c_void_p, C.c_void_p, C.POINTER(C.c_double), ERRP]),
     "lb200_pq_probe": (None, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t),
                               C.POINTER(C.c_size_t), C.c_void_p, C.c_void_p, ERRP]),
     "lb200_cast": (None, [C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_int, ERRP]),
@@ -299,6 +303,16 @@ class Index:
         s = SearchStats()
         self._call("lb200_last_search_stats", C.byref(s))
         return {f: getattr(s, f) for f, _ in SearchStats._fields_}
+
+    def screen_basis(self):
+        """(k x dims float32 basis of the projected screen, or None when the index keeps none; seconds its choice took)"""
+        sec = C.c_double()
+        k = self._call("lb200_screen_basis", None, C.byref(sec))
+        if not k:
+            return None, sec.value
+        P = np.zeros((k, self.dim), np.float32)
+        self._call("lb200_screen_basis", _ptr(P), None)
+        return P, sec.value
 
     def save_buffer(self):
         n = self._call("lb200_serialized_length")
@@ -481,6 +495,19 @@ def search_screen_probe(dataset, queries, metric="l2sq"):
     lb = np.zeros((len(Q), len(X)), np.float32)
     d = np.zeros((len(Q), len(X)), np.float32)
     _static("lb200_search_screen_probe", _ptr(X), len(X), _ptr(Q), len(Q), X.shape[1], METRIC[metric], _ptr(lb), _ptr(d))
+    return lb, d
+
+
+def search_pscreen_probe(dataset, queries, metric="l2sq", basis=None, k=0):
+    """Test hook: (lb, d), both [nq][n] float32 -- the projected screen's lower bound with `basis` (k x dims, any values) or,
+    when None, the rows' own basis of k directions (k = 0: the index's choice) -- and the search kernel's fp32 distance."""
+    X = np.ascontiguousarray(dataset, dtype=np.float32)
+    Q = np.ascontiguousarray(queries, dtype=np.float32)
+    lb = np.zeros((len(Q), len(X)), np.float32)
+    d = np.zeros((len(Q), len(X)), np.float32)
+    P = None if basis is None else np.ascontiguousarray(basis, dtype=np.float32)
+    _static("lb200_search_pscreen_probe", _ptr(X), len(X), _ptr(Q), len(Q), X.shape[1], METRIC[metric],
+            None if P is None else _ptr(P), len(P) if P is not None else k, _ptr(lb), _ptr(d))
     return lb, d
 
 

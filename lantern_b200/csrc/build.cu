@@ -367,6 +367,13 @@ void build_pending_group(Index& idx, const std::vector<BuildReplica>& replicas, 
         (void)cudaGetLastError();
         throw;
     }
+    // the search screen's choice, once the index first holds enough rows.  Its basis and records belong on the root's device:
+    // the ranks' clean-up above leaves the last rank's device current.
+    int cur = 0;
+    LB_CUDA(cudaGetDevice(&cur));
+    LB_CUDA(cudaSetDevice(replicas[root].device));
+    idx.decide_screen();
+    LB_CUDA(cudaSetDevice(cur));
 }
 
 void build_pending(Index& idx) {

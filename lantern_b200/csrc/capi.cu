@@ -326,6 +326,8 @@ LB200_EXPORT void lb200_last_search_stats(lb200_index_t h, lb200_search_stats_t*
         stats->kernel_ms = s.kernel_ms;
         stats->limbo_overflows = s.limbo_overflows;
         stats->full_rows_read = s.full_rows_read;
+        stats->screen_kind = s.screen_kind;
+        stats->screen_dims = s.screen_dims;
     });
 }
 
@@ -584,6 +586,55 @@ LB200_EXPORT void lb200_search_screen_probe(float const* dataset, size_t dataset
         LB_CUDA(cudaMemcpy(lb, dl.p, queries_size * dataset_size * 4, cudaMemcpyDeviceToHost));
         LB_CUDA(cudaMemcpy(d, dv.p, queries_size * dataset_size * 4, cudaMemcpyDeviceToHost));
     });
+}
+
+LB200_EXPORT void lb200_search_pscreen_probe(float const* dataset, size_t dataset_size, float const* queries, size_t queries_size,
+                                             size_t dimensions, lb200_metric_kind_t metric_kind, float const* basis, size_t k, float* lb,
+                                             float* d, lb200_error_t* error) {
+    guarded(error, [&] {
+        require_device();
+        check_metric_scalar(metric_kind, lb200_scalar_f32_k);
+        const int dm = distance_mode(metric_kind, SK_F32);
+        if ((dm != DM_L2SQ && dm != DM_COS) || !dimensions || !lb || !d || k > 112 || (basis && !k))
+            throw CudaError("search_pscreen_probe: needs l2sq or cos, dimensions, output buffers and k <= 112 (k >= 1 with a basis)");
+        if (!dataset_size || !queries_size)
+            return;
+        const size_t rb = round_up(dimensions * 4, 16);
+        DeviceTemp dd(dataset_size * rb), dq(queries_size * rb), dl(queries_size * dataset_size * 4), dv(queries_size * dataset_size * 4);
+        upload_rows(dataset, dataset_size, dimensions * 4, SK_F32, dimensions, dd.as<uint8_t>(), rb);
+        upload_rows(queries, queries_size, dimensions * 4, SK_F32, dimensions, dq.as<uint8_t>(), rb);
+        std::vector<float> P;
+        uint32_t kk = (uint32_t)k;
+        if (basis)
+            P.assign(basis, basis + k * dimensions);
+        else
+            kk = ps_choose_basis(dd.as<uint8_t>(), rb, dataset_size, dimensions, true, kk, P);
+        float *dP = nullptr, *dPt = nullptr;
+        struct FreeBasis {
+            float*& a;
+            float*& b;
+            ~FreeBasis() { cudaFree(a), cudaFree(b); }
+        } free_basis{dP, dPt};
+        ps_upload_basis(P, dimensions, kk, &dP, &dPt);
+        launch_pscreen_probe(dm, dd.as<uint8_t>(), dataset_size, dq.as<uint8_t>(), queries_size, (uint32_t)rb, dimensions, dP, dPt, kk,
+                             dl.as<float>(), dv.as<float>(), 0);
+        LB_CUDA(cudaMemcpy(lb, dl.p, queries_size * dataset_size * 4, cudaMemcpyDeviceToHost));
+        LB_CUDA(cudaMemcpy(d, dv.p, queries_size * dataset_size * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+LB200_EXPORT size_t lb200_screen_basis(lb200_index_t h, float* basis, double* seconds, lb200_error_t* error) {
+    size_t k = 0;
+    guarded(error, [&] {
+        Index* idx = as_index(h);
+        std::lock_guard<std::mutex> g(idx->mu_);
+        k = idx->ps_k_;
+        if (basis)
+            std::copy(idx->ps_basis_.begin(), idx->ps_basis_.end(), basis);
+        if (seconds)
+            *seconds = idx->ps_basis_ms_ / 1e3;
+    });
+    return k;
 }
 
 LB200_EXPORT void lb200_pq_probe(lb200_index_t h, int mode, float const* values, uint32_t const* nodes, size_t count, size_t* rows,

@@ -18,8 +18,6 @@ namespace lb200 {
 
 // rows up to this many bytes are searched by the warp-per-query kernel unless "search_kernel" says otherwise (0: never)
 constexpr size_t kWarpKernelMaxRowBytes = 0;
-// rows of at least this many bytes take the screened search path when the index keeps the int8 companion
-constexpr size_t kScreenMinRowBytes = 1024;
 
 std::atomic<uint64_t> g_kernel_launches{0};
 
@@ -84,6 +82,7 @@ Index::Index(const IndexConfig& cfg, const float* codebook) : cfg_(cfg) {
         row_bytes_ = round_up(vec_bytes_, 16);
         if (cfg.scalar_kind == SK_F32 && (dist_mode_ == DM_L2SQ || dist_mode_ == DM_COS))
             sq_bytes_ = screen_code_bytes((uint32_t)row_bytes_);
+        sq_on_ = sq_bytes_ != 0;
     }
     LB_CUDA(cudaMalloc(&scratch_.counters, 8 * sizeof(unsigned long long)));
     LB_CUDA(cudaMemset(scratch_.counters, 0, 8 * sizeof(unsigned long long)));
@@ -96,7 +95,8 @@ Index::~Index() {
     cudaFree(d_codebook_), cudaFree(scratch_.visited), cudaFree(scratch_.touched), cudaFree(scratch_.counters);
     cudaFree(d_query_buf_), cudaFree(d_io_buf_), cudaFree(d_warp_aux_);
     cudaFree(d_pq_pair_), cudaFree(d_pq_norm_), cudaFree(d_pending_raw_), cudaFree(d_pq_tables_);
-    cudaFree(d_sq_codes_), cudaFree(d_sq_meta_);
+    cudaFree(d_sq_codes_), cudaFree(d_sq_meta_), cudaFree(d_ps_query_);
+    free_pscreen();
     if (ev0_)
         cudaEventDestroy(ev0_);
     if (ev1_)
@@ -113,16 +113,21 @@ void Index::ensure_capacity(size_t cap) {
     grow_device(d_adj0_, n_ * cfg_.M0, nc * cfg_.M0, 0xFF);
     grow_device(d_upper_ref_, n_, nc, 0xFF);
     grow_device(d_keys_, n_, nc, 0xFF);
-    if (sq_bytes_) {
+    if (sq_on_) {
         grow_device(d_sq_codes_, used * sq_bytes_, nc * sq_bytes_, 0);
         grow_device(d_sq_meta_, used, nc, 0);
     }
+    if (ps_k_)
+        grow_device(d_ps_records_, used * ps_record_bytes(ps_k_), nc * ps_record_bytes(ps_k_), 0);
     capacity_ = nc;
 }
 
 void Index::encode_screen(size_t first, size_t count) {
-    if (sq_bytes_)
+    if (sq_on_)
         launch_sq_encode(d_vectors_ + first * row_bytes_, row_bytes_, count, d_sq_codes_ + first * sq_bytes_, d_sq_meta_ + first, 0);
+    if (ps_k_)
+        launch_ps_encode(d_vectors_ + first * row_bytes_, row_bytes_, count, cfg_.dims, d_ps_basis_, d_ps_basis_t_, ps_k_,
+                         dist_mode_ == DM_COS, d_ps_records_ + first * ps_record_bytes(ps_k_), 0);
 }
 
 void Index::reserve(size_t capacity) {
@@ -299,6 +304,8 @@ GraphView Index::view() const {
     g.pq_lut_width = pq_lut_width(cfg_.num_centroids, pq_max_code_);
     g.sq_codes = d_sq_codes_;
     g.sq_meta = d_sq_meta_;
+    g.ps_records = reinterpret_cast<const uint4*>(d_ps_records_);
+    g.ps_k = ps_k_;
     g.flags = 2u; // L2-prefetch the adjacency line of nodes that enter the top list
     if (const char* e = getenv("LB200_FLAGS"))
         g.flags = (uint32_t)atoi(e);
@@ -374,7 +381,7 @@ void Index::search_device(const void* d_queries, size_t nq, size_t stride, int k
         launch_warp_search(*this, qbuf, qrow, nq, k, (uint32_t)L, d_keys, d_dists, d_counts, stream);
         LB_CUDA(cudaEventRecord(ev1_, stream));
         last_nq_ = (uint32_t)nq;
-        last_screened_ = false;
+        last_screen_ = 0;
         return;
     }
     GraphView gv = view();
@@ -395,11 +402,33 @@ void Index::search_device(const void* d_queries, size_t nq, size_t stride, int k
             gv.pq_query_tables = d_pq_tables_;
         }
     }
-    // int8 screen of the level-0 beam (screen.cuh): below 1 KB per row the extra dependent fetch per round is unlikely to pay
-    // for the bytes it saves.  LB200_SEARCH_SCREEN=0/1 overrides the choice for experiments (same graph timed both ways).
-    bool screen = sq_bytes_ && row_bytes_ >= kScreenMinRowBytes;
-    if (const char* e = getenv("LB200_SEARCH_SCREEN"))
-        screen = sq_bytes_ && atoi(e) != 0;
+    // screen of the level-0 beam (screen.cuh): the projected one when the index chose a basis, else the int8 one; below 1 KB
+    // per row the extra dependent fetch per round is unlikely to pay for the bytes it saves.  LB200_SEARCH_SCREEN overrides
+    // the choice for experiments (one graph timed every way): 0 = off, 1 = int8, 2 = projected.  A companion the forced kind
+    // needs and the index does not keep is encoded here, before the kernel's events.
+    int screen = screen_eligible() ? (ps_auto_ ? 2 : sq_on_ ? 1 : 0) : 0;
+    if (const char* e = getenv("LB200_SEARCH_SCREEN")) {
+        const int v = atoi(e);
+        screen = !sq_bytes_ || v == 0 ? 0 : v == 2 ? 2 : 1;
+        if (screen == 1)
+            set_int8_companion(true);
+        else if (screen == 2)
+            force_pscreen();
+    }
+    gv.sq_codes = d_sq_codes_, gv.sq_meta = d_sq_meta_; // a forced kind may just have been encoded
+    gv.ps_records = reinterpret_cast<const uint4*>(d_ps_records_), gv.ps_k = ps_k_;
+    if (screen == 2) { // the batch's projections (ps_query_kernel), one dense launch
+        const size_t qbytes = nq * ps_query_floats(ps_k_) * sizeof(float);
+        if (qbytes > ps_query_bytes_) {
+            if (d_ps_query_)
+                LB_CUDA(cudaFree(d_ps_query_));
+            d_ps_query_ = nullptr;
+            ps_query_bytes_ = round_up(qbytes + qbytes / 4, 256);
+            LB_CUDA(cudaMalloc(&d_ps_query_, ps_query_bytes_));
+        }
+        launch_ps_queries(d_ps_basis_, d_ps_basis_t_, cfg_.dims, ps_k_, qbuf, qrow, nq, d_ps_query_, stream);
+        gv.ps_query = d_ps_query_;
+    }
     const uint32_t max_ctas = search_max_ctas(dist_mode_, cfg_.scalar_kind, gv, (uint32_t)L, cfg_.pq, expand, screen);
     ensure_scratch(max_ctas);
     LB_CUDA(cudaMemsetAsync(scratch_.counters, 0, 8 * sizeof(unsigned long long), stream));
@@ -418,7 +447,7 @@ void Index::search_device(const void* d_queries, size_t nq, size_t stride, int k
     launch_search(dist_mode_, cfg_.scalar_kind, cfg_.pq, p, stream);
     LB_CUDA(cudaEventRecord(ev1_, stream));
     last_nq_ = (uint32_t)nq;
-    last_screened_ = screen;
+    last_screen_ = screen;
 }
 
 void Index::search_host(const void* queries, size_t nq, size_t stride, int kind, size_t k, size_t ef, uint64_t* keys,
@@ -471,11 +500,15 @@ SearchStats Index::last_stats() {
             (void)cudaGetLastError();
     }
     s.computed_distances = c[1], s.base_pops = c[2], s.upper_hops = c[3], s.limbo_overflows = c[4];
-    const uint64_t screened = last_screened_ ? c[5] : 0, rejected = last_screened_ ? c[6] : 0;
+    const uint64_t screened = last_screen_ ? c[5] : 0, rejected = last_screen_ ? c[6] : 0;
     s.full_rows_read = s.computed_distances - rejected;
+    s.screen_kind = (uint32_t)last_screen_;
+    s.screen_dims = last_screen_ == 1 ? (uint32_t)cfg_.dims : last_screen_ == 2 ? ps_k_ : 0u;
     // SURVEY.md 8(d): B_alg = n_dist*bytes_per_stored_vector + n_pop*(4 + M_level*4) + query bytes, where a screened search
-    // reads a code row + its 16 bytes of metadata per screened candidate and a stored row only for the rest
-    s.algorithmic_bytes = screened * (sq_bytes_ + 16) + s.full_rows_read * (cfg_.pq ? stored_bytes_ : vec_bytes_) +
+    // reads a code row + its 16 bytes of metadata (int8) or one record (projected) per screened candidate and a stored row
+    // only for the rest
+    const uint64_t screen_bytes = last_screen_ == 1 ? sq_bytes_ + 16 : last_screen_ == 2 ? ps_record_bytes(ps_k_) : 0;
+    s.algorithmic_bytes = screened * screen_bytes + s.full_rows_read * (cfg_.pq ? stored_bytes_ : vec_bytes_) +
                           s.base_pops * (4 + 4 * cfg_.M0) + s.upper_hops * (4 + 4 * cfg_.M) + s.queries * vec_bytes_;
     return s;
 }

@@ -11,6 +11,8 @@
 //   keys      [capacity] u64, levels [capacity] i16
 //   sq_codes  [capacity][round_up(dims,16)] i8   f32 l2sq / cos only: the search screen's int8 copy of every row (screen.cuh)
 //   sq_meta   [capacity] float4                  {scale, bound on |x - x^|, fp32 |x|^2 as the kernel computes it, |codes|}
+//   ps_records [capacity][64 or 128]             instead of sq_*, when the index's rows fit a projected basis (pscreen.cu):
+//                                                {s, E, F, b2} then k int8 codes of P x
 //   scratch   per resident CTA: visited bitmap (capacity bits) + touched-word list
 // The reference keeps the same information in per-node byte tapes with 6-byte slots
 // (U/include/usearch/index.hpp:1799-1863); only the (de)serialiser here speaks that format.
@@ -38,6 +40,8 @@ struct IndexConfig {
 struct SearchStats {
     uint64_t queries = 0, computed_distances = 0, base_pops = 0, upper_hops = 0, algorithmic_bytes = 0, limbo_overflows = 0;
     uint64_t full_rows_read = 0; // stored rows actually read: computed_distances minus the candidates the screen rejected
+    uint32_t screen_kind = 0;    // 0 = no screen, 1 = int8 codes, 2 = projected codes
+    uint32_t screen_dims = 0;    // codes per screened candidate: dims (int8) or k (projected)
     double kernel_ms = 0; // device time of the search kernel alone (CUDA events on the launching stream)
 };
 
@@ -64,7 +68,23 @@ struct GraphView {
     // search screen (f32 l2sq / cos): int8 code rows of screen_code_bytes(row_bytes) and their metadata, or NULL
     const uint8_t* sq_codes;
     const float4* sq_meta;
+    // projected screen: records of ps_record_bytes(ps_k), and the search batch's pre-pass (ps_query_floats(ps_k) per query)
+    const uint4* ps_records;
+    const float* ps_query;
+    uint32_t ps_k;
 };
+
+// The projected screen's basis (pscreen.cu): chosen from the first build (or load) that leaves kPsMinRows rows, as the smallest
+// k of kPsDims whose mean residual energy |x - P^T P x|^2 / |x|^2 over a sample of at most kPsSampleMax rows is <= kPsMaxResidual
+constexpr size_t kPsMinRows = 16384;
+constexpr size_t kPsSampleMax = 65536;
+constexpr double kPsMaxResidual = 0.01;
+constexpr uint32_t kPsDims[] = {16, 32, 48, 64, 96, 112};
+// above 256 dimensions the top eigenvectors come from subspace iteration with this many vectors and iterations (pscreen.cu)
+constexpr size_t kPsSubspace = 128;
+constexpr int kPsSubspaceIters = 12;
+// rows of at least this many bytes take a screened search path when the index keeps a companion
+constexpr size_t kScreenMinRowBytes = 1024;
 
 // Floats of one value's PQ look-up table: [nsub][lut_width] padded to whole 16-byte chunks, then |value|^2 and 3 spare floats.
 // Precomputed tables travel to shared memory by bulk copy, whose size and addresses must be multiples of 16 bytes.
@@ -165,8 +185,20 @@ class Index {
     // search screen companion (f32 storage, l2sq / cos, not PQ): written from d_vectors_ by launch_sq_encode
     uint8_t* d_sq_codes_ = nullptr;
     float4* d_sq_meta_ = nullptr;
-    size_t sq_bytes_ = 0; // bytes of one code row; 0 = this index keeps no companion
-    bool last_screened_ = false;
+    size_t sq_bytes_ = 0; // bytes of one code row; 0 = this index cannot keep the int8 companion
+    bool sq_on_ = false;  // the int8 companion is allocated and kept up to date
+    // projected screen (pscreen.cu): basis [k][dims] (host), device P [slots][dims] and P^T [dims][slots], records [capacity]
+    uint32_t ps_k_ = 0; // 0 = no basis
+    std::vector<float> ps_basis_;
+    float* d_ps_basis_ = nullptr;
+    float* d_ps_basis_t_ = nullptr;
+    uint8_t* d_ps_records_ = nullptr;
+    float* d_ps_query_ = nullptr; // the search batch's pre-pass
+    size_t ps_query_bytes_ = 0;
+    bool ps_decided_ = false;  // the automatic choice has been made
+    bool ps_auto_ = false;     // ... and it is the projected screen (a basis may also exist because LB200_SEARCH_SCREEN=2 forced one)
+    double ps_basis_ms_ = 0;   // host time of the last basis choice (moment matrix, eigenvectors, records)
+    int last_screen_ = 0;      // screen kind of the last search
     size_t pending_raw_cap_ = 0;
     // host mirrors of the small per-node metadata
     std::vector<int16_t> h_levels_;
@@ -198,7 +230,15 @@ class Index {
     void ensure_scratch(uint32_t ctas);
     // throws unless a PQ walk with a look-up table `lut_width` centroids wide fits in one CTA's shared memory
     void check_pq_table_fits(uint32_t lut_width) const;
-    void encode_screen(size_t first, size_t count); // companion of rows [first, first + count) from d_vectors_
+    void encode_screen(size_t first, size_t count); // companions of rows [first, first + count) from d_vectors_
+    // the search screen's choice (pscreen.cu)
+    bool screen_eligible() const; // f32 l2sq / cos rows of >= kScreenMinRowBytes
+    void decide_screen();         // automatic choice, once rows >= kPsMinRows (after a build, after load_buffer)
+    void reset_screen();          // load_buffer: forget the choice, int8 companion back on
+    void force_pscreen();         // a basis for LB200_SEARCH_SCREEN=2 when there is none
+    void set_pscreen_basis(const std::vector<float>& P, uint32_t k);
+    void set_int8_companion(bool on);
+    void free_pscreen();
     void* io_buffer(size_t bytes);
     uint8_t* query_buffer(size_t bytes);
 };
@@ -217,6 +257,15 @@ void launch_pq_query_tables(const float* d_codebook, size_t dims, size_t nsub, s
                             size_t q_stride_floats, size_t nq, float* d_tables, cudaStream_t stream);
 // screen.cuh companion of n stored f32 rows (row_bytes apart): codes[n][screen_code_bytes(row_bytes)], meta[n]
 void launch_sq_encode(const uint8_t* d_rows, size_t row_bytes, size_t n, uint8_t* d_codes, float4* d_meta, cudaStream_t stream);
+// pscreen.cu: records of n stored f32 rows for the basis (d_P [slots][dims], d_Pt [dims][slots]); the pre-pass of nq queries
+// (storage rows q_stride apart) into d_out[nq][ps_query_floats(k)]; device copies of a host basis [k][dims]; the basis choice
+void launch_ps_encode(const uint8_t* d_rows, size_t row_bytes, size_t n, size_t dims, const float* d_P, const float* d_Pt, uint32_t k,
+                      bool cosine, uint8_t* d_records, cudaStream_t stream);
+void launch_ps_queries(const float* d_P, const float* d_Pt, size_t dims, uint32_t k, const uint8_t* d_queries, size_t q_stride, size_t nq,
+                       float* d_out, cudaStream_t stream);
+void ps_upload_basis(const std::vector<float>& P, size_t dims, uint32_t k, float** d_P, float** d_Pt);
+// want_k = 0: the smallest qualifying k (0 = none; `force`: the best one); else the top want_k eigenvectors
+uint32_t ps_choose_basis(const uint8_t* d_rows, size_t row_bytes, size_t n, size_t dims, bool force, uint32_t want_k, std::vector<float>& P);
 void launch_pq_decode(const float* d_codebook, size_t dims, size_t ncent, size_t nsub, const uint8_t* d_codes,
                       size_t code_stride, size_t n, float* d_vecs, cudaStream_t stream);
 // search.cu
@@ -227,16 +276,19 @@ struct SearchLaunch {
     uint32_t query_stride;
     uint32_t nq, k, L;
     uint32_t expand; // candidates expanded per round (1 = the reference's exact order)
-    bool screen;     // level-0 beam screens candidates with g.sq_codes before reading their rows (screen.cuh)
+    int screen;      // level-0 beam screens candidates before reading their rows (screen.cuh): 1 = g.sq_codes, 2 = g.ps_records
     uint64_t* out_keys;
     float* out_dists;
     uint32_t* out_counts;
 };
-uint32_t search_max_ctas(int dist_mode, int scalar_kind, const GraphView& g, uint32_t L, bool pq, uint32_t expand, bool screen);
+uint32_t search_max_ctas(int dist_mode, int scalar_kind, const GraphView& g, uint32_t L, bool pq, uint32_t expand, int screen);
 // test hook: screen bound and the search kernel's own fp32 distance for every (query, row) pair; device rows / queries
 // row_bytes apart, outputs [nq][n]
 void launch_screen_probe(int dist_mode, const uint8_t* d_rows, size_t n, const uint8_t* d_queries, size_t nq, uint32_t row_bytes,
                          float* d_lb, float* d_dist, cudaStream_t stream);
+// the same for the projected screen with the basis d_P / d_Pt of k rows
+void launch_pscreen_probe(int dist_mode, const uint8_t* d_rows, size_t n, const uint8_t* d_queries, size_t nq, uint32_t row_bytes,
+                          size_t dims, const float* d_P, const float* d_Pt, uint32_t k, float* d_lb, float* d_dist, cudaStream_t stream);
 void launch_search(int dist_mode, int scalar_kind, bool pq, const SearchLaunch& p, cudaStream_t stream);
 // test hook: PqEval on the view `g` of a PQ index, for `count` values -- raw f32 rows value_stride bytes apart (tables from
 // g.pq_query_tables when set, else built in the kernel), or stored nodes when d_nodes != NULL.  Outputs d_dist[count][g.n]

@@ -237,6 +237,7 @@ void Index::load_buffer(const void* buffer, size_t length) {
     pq_max_code_ = pq_max_code;
     n_ = 0, pending_n_ = 0;
     ensure_capacity(n ? n : 1);
+    reset_screen(); // the screen is chosen again from the loaded rows
     upper_lists_ = 0;
     alloc_upper(upper_adj.size() / M + 1);
     // everything beyond the loaded nodes / lists must read as empty (0xFF): a later insert with level > max_level exposes
@@ -259,6 +260,7 @@ void Index::load_buffer(const void* buffer, size_t length) {
     n_ = n;
     max_level_ = n ? (int32_t)hdr[3] : -1;
     entry_ = (uint32_t)hdr[4];
+    decide_screen();
 }
 
 } // namespace lb200

@@ -1287,7 +1287,7 @@ static std::unique_ptr<Index> build_replica(Index& root) {
         LB_CUDA(cudaMemcpy(codebook.data(), root.d_codebook_, codebook.size() * sizeof(float), cudaMemcpyDeviceToHost));
     }
     std::unique_ptr<Index> x(new Index(cfg, codebook.data()));
-    x->sq_bytes_ = 0;
+    x->sq_bytes_ = 0, x->sq_on_ = false;
     x->ensure_capacity(root.capacity_);
     x->alloc_upper(root.upper_lists_);
     const size_t n0 = root.n_, P = root.pending_n_;

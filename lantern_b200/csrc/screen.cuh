@@ -93,4 +93,67 @@ template <int DM, int NQ> __device__ __forceinline__ float screen_bound(float s,
 }
 #endif
 
+// ---- the projected screen (DESIGN.md 4.1): k int8 codes of y = P x instead of one per dimension -------------------------
+// P is a k x dims fp32 basis chosen per index (pscreen.cu); nothing below assumes it is orthonormal, so any P gives a valid
+// bound.  One record per row: ps_meta = {s, E >= |e|, F >= |P e|, b2} (e = x - P^T s c), then `ps_code_slots` int8 codes
+// (zero beyond k).  b2 is the kernel's own fp32 |x|^2 (cos) or a rounded-down |x|^2 (l2sq).
+LB_HD inline uint32_t ps_record_bytes(uint32_t k) { return k <= 48 ? 64u : 128u; }
+LB_HD inline uint32_t ps_code_slots(uint32_t k) { return ps_record_bytes(k) - 16u; }
+// per query, written once per batch: q~ = fl(P q) in `ps_code_slots` floats (zero beyond k), then
+// {delta >= |P q - q~|, >= |q~|, G >= |q - P^T q~|, <= |q|^2}
+LB_HD inline uint32_t ps_query_floats(uint32_t k) { return ps_code_slots(k) + 4u; }
+
+#ifdef __CUDACC__
+// lb <= the distance row_distance<DM, SK_F32, NQ> computes for the query (registers, a2) and the row, from
+//   sf = fl(sum_j q~_j c_j) (`slots` chained fma), cc = sum_j c_j^2 (exact in fp32: < 2^24), the row's meta, the query's header.
+// q.x = q~.y^ + (Pq - q~).y^ + q~.(P e) + (q - P^T q~).e  <=  s sf + screen rounding + delta |y^| + |q~| F + G E  (y^ = s c)
+template <int DM, int NQ>
+__device__ __forceinline__ float pscreen_bound(float sf, float cc, float4 meta, float4 qh, float a2, uint32_t slots) {
+    const double s = meta.x, E = meta.y, F = meta.z;
+    const float b2 = meta.w;
+    const double cn = sqrt((double)cc) * (1.0 + 0x1p-50);    // |c|
+    const double qt = qh.y;                                   // >= |q~|
+    const double A = s * (double)sf;                          // exact: 24 x 24 bits
+    // screen: |sf - q~.c| <= gamma(slots) |q~||c| + kSubAbs; then delta |y^|, |q~| F, G E
+    double B = s * (gamma32((int)slots) * qt * cn + kSubAbs) + (double)qh.x * (s * cn) + qt * F + (double)qh.z * E;
+    if constexpr (DM == DM_COS) {
+        if (!(a2 > 0.f) || !(b2 > 0.f) || !(a2 < 0x1p126f) || !(b2 < 0x1p126f))
+            return -INFINITY;
+        // the kernel's fp32 dot product: |ab_k - q.x| <= gamma(2 NQ + 6) |q||x| + kSubAbs, |q|, |x| from its own a2, b2
+        const double qn = sqrt(((double)a2 + kSubAbs) * (1.0 + gamma32(NQ + 9))) * (1.0 + 0x1p-50);
+        const double xn = sqrt(((double)b2 + kSubAbs) * (1.0 + gamma32(NQ + 9))) * (1.0 + 0x1p-50);
+        B += gamma32(2 * NQ + 6) * qn * xn + kSubAbs;
+    }
+    if (!(fabs(A) < INFINITY) || !(B < INFINITY)) // NaN / inf anywhere (non-finite data, overflow): cannot tell
+        return -INFINITY;
+    const double Bp = B * (1.0 + 0x1p-45); // the double roundings of B
+    const double U = (A + Bp) + (fabs(A) + Bp) * 0x1p-50;
+    if constexpr (DM == DM_COS) {
+        // the final arithmetic replayed, as screen_bound does
+        return __fsub_rn(1.f, __fdiv_rn(__double2float_ru(U), __fmul_rn(sqrtf(a2), sqrtf(b2))));
+    } else {
+        // |q - x|^2 = |q|^2 - 2 q.x + |x|^2 >= qq - 2U + b2 (three double roundings bounded below), then the kernel's sum as in
+        // screen_bound: d >= (1 - gamma(NQ + 9)) |q - x|^2 - kSubAbs
+        const double qq = qh.w;
+        const double D = (qq - 2.0 * U) + (double)b2;
+        const double L2 = D - (qq + 2.0 * fabs(U) + (double)b2) * 0x1p-50;
+        const double lb = fmax(L2, 0.0) * (1.0 - gamma32(NQ + 9)) * (1.0 - 0x1p-46) - kSubAbs;
+        return __double2float_rd(lb);
+    }
+}
+
+// fl(sum_j q~_j c_j) and sum_j c_j^2 over one 16-byte group of codes, q~ from shared memory
+__device__ __forceinline__ void ps_accum(const float* qt, uint4 w, float& sf, float& cc) {
+    const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int b = 0; b < 4; ++b) {
+            const float c = (float)(int8_t)(ws[i] >> (8 * b));
+            sf = __fmaf_rn(qt[4 * i + b], c, sf);
+            cc = __fmaf_rn(c, c, cc);
+        }
+}
+#endif
+
 } // namespace lb200

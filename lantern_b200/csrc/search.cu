@@ -117,6 +117,38 @@ __global__ void __launch_bounds__(128) screen_probe_kernel(const uint8_t* rows, 
     }
 }
 
+// test hook (lb200_search_pscreen_probe): the projected screen's bound, through PScreenEval's own per-candidate arithmetic
+// (records, q~ in shared memory, pscreen_bound), and row_distance() for every (query, row) pair.  One CTA per query, one
+// lane per row for the bound, one warp per row for the distance.
+template <int DM, int NQ>
+__global__ void __launch_bounds__(128) pscreen_probe_kernel(const uint8_t* rows, uint32_t n, const uint8_t* queries, uint32_t row_bytes,
+                                                            const uint4* records, const float* qpre, uint32_t k, float* out_lb,
+                                                            float* out_d) {
+    __shared__ float psq[128];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t nchunks = row_bytes / 16, slots = ps_code_slots(k), rec = ps_record_bytes(k) / 16, nf = ps_query_floats(k);
+    for (uint32_t i = threadIdx.x; i < nf; i += blockDim.x)
+        psq[i] = qpre[(size_t)blockIdx.x * nf + i];
+    __syncthreads();
+    uint4 qreg[NQ];
+    const float a2 = load_qreg<DM, SK_F32, NQ>(qreg, queries + (size_t)blockIdx.x * row_bytes, nchunks, lane);
+    const float4 qh = *reinterpret_cast<const float4*>(psq + slots);
+    for (uint32_t j = threadIdx.x; j < n; j += blockDim.x) {
+        const uint4* r = records + (size_t)j * rec;
+        float sf = 0.f, cc = 0.f;
+        for (uint32_t g = 1; g < rec; ++g)
+            ps_accum(psq + 16 * (g - 1), __ldg(r + g), sf, cc);
+        const uint4 v0 = __ldg(r);
+        const float4 meta = make_float4(__uint_as_float(v0.x), __uint_as_float(v0.y), __uint_as_float(v0.z), __uint_as_float(v0.w));
+        out_lb[(size_t)blockIdx.x * n + j] = pscreen_bound<DM, NQ>(sf, cc, meta, qh, a2, slots);
+    }
+    for (uint32_t j = warp; j < n; j += blockDim.x / 32) {
+        const float d = row_distance<DM, SK_F32, NQ>(qreg, reinterpret_cast<const uint4*>(rows + (size_t)j * row_bytes), nchunks, a2, lane);
+        if (lane == 0)
+            out_d[(size_t)blockIdx.x * n + j] = d;
+    }
+}
+
 // test hook (lb200_pq_probe): the walkers' own PqEval<DM> on the index's view.  CTA v turns value v into its look-up table
 // (load_query: the batch's precomputed tables when g.pq_query_tables is set, else load_value; load_node for node values),
 // copies the table and |v|^2 out, then measures every stored row through eval(), cand_cap rows per pass, as a walk does.
@@ -177,13 +209,17 @@ template <class W> int occupancy_one(size_t smem, int threads) {
     return blocks;
 }
 
-// fn(walker type tag) with the screened walker of an f32 l2sq / cos index
-template <typename Fn> void dispatch_screen(int dm, int nq, Fn&& fn) {
+// fn(walker type tag) with the screened walker of an f32 l2sq / cos index: 1 = int8 codes, 2 = projected codes
+template <typename Fn> void dispatch_screen(int screen, int dm, int nq, Fn&& fn) {
     dispatch_walk(dm, SK_F32, nq, [&](auto d, auto s, auto n) {
-        if constexpr (decltype(s)::value == SK_F32 && (decltype(d)::value == DM_L2SQ || decltype(d)::value == DM_COS))
-            fn(TypeTag<ScreenWalker<decltype(d)::value, decltype(n)::value>>{});
-        else
+        if constexpr (decltype(s)::value == SK_F32 && (decltype(d)::value == DM_L2SQ || decltype(d)::value == DM_COS)) {
+            if (screen == 2)
+                fn(TypeTag<PScreenWalker<decltype(d)::value, decltype(n)::value>>{});
+            else
+                fn(TypeTag<ScreenWalker<decltype(d)::value, decltype(n)::value>>{});
+        } else {
             throw CudaError("search screen: f32 l2sq / cos indexes only");
+        }
     });
 }
 
@@ -201,22 +237,25 @@ static int search_threads(const GraphView& g, bool pq) {
     return warps * 32;
 }
 
-static size_t search_smem(const GraphView& g, bool pq, uint32_t R, uint32_t L, uint32_t expand) {
-    return pq ? walk_layout_pq(g.num_subvectors, g.pq_lut_width, pq_value_floats(g), L, g.M0 * expand).total
-              : walk_layout(R, g.row_bytes, L, g.M0 * expand).total;
+static size_t search_smem(const GraphView& g, bool pq, int screen, uint32_t R, uint32_t L, uint32_t expand) {
+    if (pq)
+        return walk_layout_pq(g.num_subvectors, g.pq_lut_width, pq_value_floats(g), L, g.M0 * expand).total;
+    if (screen == 2)
+        return PScreenEval<DM_L2SQ, 1>::layout(g, R, L, g.M0 * expand).total; // the same for every (DM, NQ)
+    return walk_layout(R, g.row_bytes, L, g.M0 * expand).total;
 }
 
-uint32_t search_max_ctas(int dist_mode, int scalar_kind, const GraphView& g, uint32_t L, bool pq, uint32_t expand, bool screen) {
+uint32_t search_max_ctas(int dist_mode, int scalar_kind, const GraphView& g, uint32_t L, bool pq, uint32_t expand, int screen) {
     const uint32_t R = pick_ring_slots(g.row_bytes);
     const int nq = pq ? 1 : pick_nq(g.row_bytes);
     if (nq < 0)
         throw CudaError("search: vectors wider than 8192 bytes are not supported");
-    const size_t smem = search_smem(g, pq, R, L, expand);
+    const size_t smem = search_smem(g, pq, screen, R, L, expand);
     int occ = 0;
     const int threads = search_threads(g, pq);
     auto occ_fn = [&](auto tag) { occ = occupancy_one<typename decltype(tag)::type>(smem, threads); };
     if (screen)
-        dispatch_screen(dist_mode, nq, occ_fn);
+        dispatch_screen(screen, dist_mode, nq, occ_fn);
     else
         dispatch_walker(pq, dist_mode, scalar_kind, nq, occ_fn);
     if (occ < 1)
@@ -227,12 +266,12 @@ uint32_t search_max_ctas(int dist_mode, int scalar_kind, const GraphView& g, uin
 void launch_search(int dist_mode, int scalar_kind, bool pq, const SearchLaunch& p, cudaStream_t stream) {
     const uint32_t R = pick_ring_slots(p.g.row_bytes);
     const int nq = pq ? 1 : pick_nq(p.g.row_bytes);
-    const size_t smem = search_smem(p.g, pq, R, p.L, p.expand);
+    const size_t smem = search_smem(p.g, pq, p.screen, R, p.L, p.expand);
     const uint32_t grid = p.s.ctas < p.nq ? p.s.ctas : p.nq;
     const int threads = search_threads(p.g, pq);
     auto launch_fn = [&](auto tag) { launch_one<typename decltype(tag)::type>(p, R, smem, grid, threads, stream); };
     if (p.screen)
-        dispatch_screen(dist_mode, nq, launch_fn);
+        dispatch_screen(p.screen, dist_mode, nq, launch_fn);
     else
         dispatch_walker(pq, dist_mode, scalar_kind, nq, launch_fn);
 }
@@ -271,6 +310,43 @@ void launch_screen_probe(int dist_mode, const uint8_t* d_rows, size_t n, const u
         throw;
     }
     cudaFree(codes), cudaFree(meta);
+}
+
+void launch_pscreen_probe(int dist_mode, const uint8_t* d_rows, size_t n, const uint8_t* d_queries, size_t nq, uint32_t row_bytes,
+                          size_t dims, const float* d_P, const float* d_Pt, uint32_t k, float* d_lb, float* d_dist, cudaStream_t stream) {
+    const int nqr = pick_nq(row_bytes);
+    if (nqr < 0)
+        throw CudaError("pscreen probe: vectors wider than 8192 bytes are not supported");
+    if (!n || !nq)
+        return;
+    uint8_t* records = nullptr;
+    float* qpre = nullptr;
+    LB_CUDA(cudaMalloc(&records, n * ps_record_bytes(k)));
+    cudaError_t e = cudaMalloc(&qpre, nq * ps_query_floats(k) * sizeof(float));
+    if (e != cudaSuccess) {
+        cudaFree(records);
+        LB_CUDA(e);
+    }
+    try {
+        launch_ps_encode(d_rows, row_bytes, n, dims, d_P, d_Pt, k, dist_mode == DM_COS, records, stream);
+        launch_ps_queries(d_P, d_Pt, dims, k, d_queries, row_bytes, nq, qpre, stream);
+        dispatch_walk(dist_mode, SK_F32, nqr, [&](auto d, auto s, auto q) {
+            constexpr int DM = decltype(d)::value;
+            if constexpr (decltype(s)::value == SK_F32 && (DM == DM_L2SQ || DM == DM_COS)) {
+                pscreen_probe_kernel<DM, decltype(q)::value><<<(unsigned)nq, 128, 0, stream>>>(
+                    d_rows, (uint32_t)n, d_queries, row_bytes, reinterpret_cast<const uint4*>(records), qpre, k, d_lb, d_dist);
+                LB_CUDA(cudaGetLastError());
+                count_launch();
+            } else {
+                throw CudaError("pscreen probe: l2sq or cos only");
+            }
+        });
+        LB_CUDA(cudaStreamSynchronize(stream));
+    } catch (...) {
+        cudaFree(records), cudaFree(qpre);
+        throw;
+    }
+    cudaFree(records), cudaFree(qpre);
 }
 
 void launch_pq_probe(int dist_mode, const GraphView& g, uint32_t cand_cap, const uint8_t* d_values, uint32_t value_stride,

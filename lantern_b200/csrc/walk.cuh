@@ -326,6 +326,29 @@ template <int DM, int SK, int NQ> struct RowEval : WalkBase {
     }
 };
 
+// Screened walkers: after cand_d[0..n) holds every candidate's lower bound, warp 0 keeps, in stored order, the candidates with
+// !(lb >= radius); returns their number (uniform across the CTA)
+__device__ __forceinline__ uint32_t screen_compact(WalkSmem& sm, uint32_t n, float radius, int warp, int lane) {
+    __syncthreads();
+    if (warp == 0) {
+        uint32_t m = 0;
+        for (uint32_t base = 0; base < n; base += 32) {
+            const uint32_t j = base + lane;
+            const bool keep = j < n && !(sm.cand_d[j] >= radius);
+            const uint32_t id = j < n ? sm.cand_id[j] : 0u;
+            const uint32_t mk = __ballot_sync(0xffffffffu, keep);
+            __syncwarp();
+            if (keep)
+                sm.cand_id[m + __popc(mk & ((1u << lane) - 1u))] = id;
+            m += __popc(mk);
+        }
+        if (lane == 0)
+            sm.ctrl->m = m, sm.ctrl->screened += n, sm.ctrl->rejected += n - m;
+    }
+    __syncthreads();
+    return sm.ctrl->m;
+}
+
 // ---- f32 rows with the int8 screen (screen.cuh, DESIGN.md 4.1): the search kernel's evaluator for l2sq / cos -------------
 // screen(n, radius) runs between the compaction of a round's unseen candidates and eval(): every warp fetches the code rows
 // of its candidates (j % NW == warp) into its own ring slots with bulk copies, all issued before the first wait, computes
@@ -386,24 +409,67 @@ template <int DM, int NQ> struct ScreenEval : RowEval<DM, SK_F32, NQ> {
                 sm.cand_d[warp + NW * (t0 + lane)] = screen_bound<DM, NQ>(mine, meta, this->a2);
         }
         fence_proxy_async(); // the code reads precede eval's bulk copies into the same slots
+        return screen_compact(sm, n, radius, warp, lane);
+    }
+};
+
+// ---- f32 rows with the projected screen (screen.cuh, DESIGN.md 4.1): k int8 codes of P x per row ---------------------------
+// Same place in the round and the same compaction as ScreenEval, but each lane takes one candidate of its warp (j % NW ==
+// warp) and reads its whole record (64 or 128 bytes) with plain 16-byte loads: one round trip for up to 32 candidates, q~
+// broadcast from shared memory, no shuffles and no ring slots.  eval() is untouched.
+template <int DM, int NQ> struct PScreenEval : RowEval<DM, SK_F32, NQ> {
+    using Base = RowEval<DM, SK_F32, NQ>;
+    static constexpr bool kScreen = true;
+    static constexpr int kMinCtas = ScreenEval<DM, NQ>::kMinCtas;
+    // the ring, then the query's q~ and its header (ps_query_floats)
+    static __host__ __device__ WalkLayout layout(const GraphView& g, uint32_t R, uint32_t top_cap, uint32_t cand_cap) {
+        return walk_layout_bytes((size_t)R * g.row_bytes + (size_t)ps_query_floats(g.ps_k) * 4, R, top_cap, cand_cap);
+    }
+    float* psq; // shared: q~[ps_code_slots], then {delta, |q~|, G, |q|^2}
+
+    __device__ __forceinline__ explicit PScreenEval(const GraphView& gv) : Base(gv) {}
+    __device__ __forceinline__ void init(uint8_t* smem_raw, const WalkLayout& lay, uint32_t ring_slots, const SearchScratch& s) {
+        Base::init(smem_raw, lay, ring_slots, s);
+        psq = reinterpret_cast<float*>(smem_raw + (size_t)ring_slots * this->g.row_bytes);
+        if (threadIdx.x == 0)
+            this->sm.ctrl->screened = this->sm.ctrl->rejected = 0; // read back after the CTA's last barrier
+    }
+    // the query's registers, and its projection from the batch's pre-pass (launch_ps_queries)
+    __device__ __forceinline__ void load_query(uint32_t qi, const uint8_t* row) {
+        Base::load_value(row);
+        const uint32_t nf = ps_query_floats(this->g.ps_k);
+        __syncthreads(); // the previous query's screen is done with psq
+        for (uint32_t i = threadIdx.x; i < nf; i += blockDim.x)
+            psq[i] = __ldg(this->g.ps_query + (size_t)qi * nf + i);
         __syncthreads();
-        if (warp == 0) {
-            uint32_t m = 0;
-            for (uint32_t base = 0; base < n; base += 32) {
-                const uint32_t j = base + lane;
-                const bool keep = j < n && !(sm.cand_d[j] >= radius);
-                const uint32_t id = j < n ? sm.cand_id[j] : 0u;
-                const uint32_t mk = __ballot_sync(0xffffffffu, keep);
-                __syncwarp();
-                if (keep)
-                    sm.cand_id[m + __popc(mk & ((1u << lane) - 1u))] = id;
-                m += __popc(mk);
+    }
+
+    __device__ __forceinline__ uint32_t screen(uint32_t n, float radius) {
+        const GraphView& g = this->g;
+        WalkSmem& sm = this->sm;
+        const int warp = this->warp, lane = this->lane;
+        const uint32_t NW = this->NW, slots = ps_code_slots(g.ps_k), rec = ps_record_bytes(g.ps_k) / 16;
+        const uint32_t T = n > (uint32_t)warp ? (n - warp + NW - 1) / NW : 0;
+        const float4 qh = *reinterpret_cast<const float4*>(psq + slots);
+        for (uint32_t t = lane; t < T; t += 32) {
+            const uint32_t j = warp + NW * t;
+            const uint4* r = g.ps_records + (size_t)sm.cand_id[j] * rec;
+            float sf = 0.f, cc = 0.f;
+            const uint4 v0 = __ldg(r), v1 = __ldg(r + 1), v2 = __ldg(r + 2), v3 = __ldg(r + 3);
+            ps_accum(psq, v1, sf, cc);
+            ps_accum(psq + 16, v2, sf, cc);
+            ps_accum(psq + 32, v3, sf, cc);
+            if (rec == 8) { // k > 48: the record's second half
+                const uint4 v4 = __ldg(r + 4), v5 = __ldg(r + 5), v6 = __ldg(r + 6), v7 = __ldg(r + 7);
+                ps_accum(psq + 48, v4, sf, cc);
+                ps_accum(psq + 64, v5, sf, cc);
+                ps_accum(psq + 80, v6, sf, cc);
+                ps_accum(psq + 96, v7, sf, cc);
             }
-            if (lane == 0)
-                sm.ctrl->m = m, sm.ctrl->screened += n, sm.ctrl->rejected += n - m;
+            const float4 meta = make_float4(__uint_as_float(v0.x), __uint_as_float(v0.y), __uint_as_float(v0.z), __uint_as_float(v0.w));
+            sm.cand_d[j] = pscreen_bound<DM, NQ>(sf, cc, meta, qh, this->a2, slots);
         }
-        __syncthreads();
-        return sm.ctrl->m;
+        return screen_compact(sm, n, radius, warp, lane);
     }
 };
 
@@ -892,6 +958,7 @@ template <class E> struct WalkerT : E {
 template <int DM, int SK, int NQ> using Walker = WalkerT<RowEval<DM, SK, NQ>>;
 template <int DM> using PqWalker = WalkerT<PqEval<DM>>;
 template <int DM, int NQ> using ScreenWalker = WalkerT<ScreenEval<DM, NQ>>;
+template <int DM, int NQ> using PScreenWalker = WalkerT<PScreenEval<DM, NQ>>;
 
 // ---- (DM, SK, NQ) dispatch shared by the launchers ----------------------------------------------------
 // PQ indexes: fn(walker type tag) with PqWalker<DM>

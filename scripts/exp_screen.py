@@ -1,10 +1,14 @@
-"""Dev experiment: the int8 search screen on vs off (LB200_SEARCH_SCREEN) on ONE built graph (needs a GPU).
+"""Dev experiment: the search screens (LB200_SEARCH_SCREEN 0 = off, 1 = int8, 2 = projected) on ONE built graph (needs a GPU).
 
-Builds a workload's graph once with bench.py's generator and seeds, then alternates the knob 0/1 for ROUNDS rounds of STEPS
-timed search steps each.  Prints, per setting, queries/s (median and spread over the rounds), kernel time, the share of
-candidates read in full (full_rows_read / computed_distances), that both settings return identical keys, distances and
-counters, and the device memory in use after the build and after the first search.
-usage: python scripts/exp_screen.py [workload] ; env ROUNDS (default 3), STEPS (default 20), OUT (directory for the JSON)"""
+Builds a workload's graph once with bench.py's generator and seeds (DATA=gauss: isotropic Gaussian rows and queries instead),
+then alternates the knobs for ROUNDS rounds of STEPS timed search steps each.  Prints, per setting, queries/s (median and
+spread over the rounds), kernel time, the share of candidates read in full (full_rows_read / computed_distances), the screen
+kind and codes per candidate, that every setting returns identical keys, distances and counters, and the device memory in use
+after the build (with the automatically chosen companion) and after each setting's first search (a forced kind encodes its
+companion then).
+usage: python scripts/exp_screen.py [workload] ; env ROUNDS (default 3), STEPS (default 20), KNOBS (default 0,1,2; "auto" =
+unset),
+DATA (structured | gauss), OUT (directory for the JSON)"""
 import json, os, sys, time
 sys.path.insert(0, '.')
 import numpy as np, torch
@@ -14,12 +18,18 @@ from lantern_b200 import api
 wl_name = sys.argv[1] if len(sys.argv) > 1 else "cfg3"
 wl = bench.WORKLOADS[wl_name]
 rounds, steps = int(os.environ.get("ROUNDS", "3")), int(os.environ.get("STEPS", "20"))
+knobs = os.environ.get("KNOBS", "0,1,2").split(",")
+data = os.environ.get("DATA", "structured")
 n, dim, B, k, ef = wl["n"], wl["dim"], wl["batch"], wl["k"], wl["ef"]
 dev = torch.device("cuda", 0)
 free0, total = torch.cuda.mem_get_info()
-X = bench.structured_torch(n, dim, bench.SEED_CORPUS, dev)
 pool = 4
-Q = bench.structured_torch(pool * B, dim, bench.SEED_QUERY, dev)
+if data == "gauss":
+    X = torch.randn((n, dim), generator=torch.Generator(device=dev).manual_seed(bench.SEED_CORPUS), device=dev)
+    Q = torch.randn((pool * B, dim), generator=torch.Generator(device=dev).manual_seed(bench.SEED_QUERY), device=dev)
+else:
+    X = bench.structured_torch(n, dim, bench.SEED_CORPUS, dev)
+    Q = bench.structured_torch(pool * B, dim, bench.SEED_QUERY, dev)
 idx = api.Index(dim, wl["metric"], "f32", M=wl["M"], efc=wl["efc"], ef=ef)
 idx.reserve(n)
 t = time.time()
@@ -28,7 +38,10 @@ idx.build()
 torch.cuda.synchronize()
 mem = {"total_gb": total / 1e9, "used_before_gb": (total - free0) / 1e9}
 mem["used_after_build_gb"] = (total - torch.cuda.mem_get_info()[0]) / 1e9
-print("%s: build %.1f s" % (wl_name, time.time() - t), flush=True)
+basis, basis_s = idx.screen_basis()
+mem["basis_seconds"] = basis_s
+print("%s (%s): build %.1f s, basis k=%s (%.2f s)" % (wl_name, data, time.time() - t, None if basis is None else len(basis), basis_s),
+      flush=True)
 ok = torch.empty((B, k), dtype=torch.int64, device=dev)
 od = torch.empty((B, k), dtype=torch.float32, device=dev)
 oc = torch.empty((B,), dtype=torch.int32, device=dev)
@@ -41,8 +54,11 @@ def step(s):
 
 
 ref = {}
-for knob in ("0", "1"):  # outputs and counters of every pool batch, both ways
-    os.environ["LB200_SEARCH_SCREEN"] = knob
+for knob in ["auto"] + knobs:  # outputs and counters of every pool batch, every way
+    if knob == "auto":
+        os.environ.pop("LB200_SEARCH_SCREEN", None)
+    else:
+        os.environ["LB200_SEARCH_SCREEN"] = knob
     outs = []
     t = time.time()
     for s in range(pool):
@@ -50,17 +66,22 @@ for knob in ("0", "1"):  # outputs and counters of every pool batch, both ways
         torch.cuda.synchronize()
         st = idx.last_stats()
         outs.append((ok.cpu().numpy().copy(), od.cpu().numpy().view(np.uint32).copy(), oc.cpu().numpy().copy(),
-                     st["computed_distances"], st["base_pops"], st["upper_hops"], st["full_rows_read"]))
+                     st["computed_distances"], st["base_pops"], st["upper_hops"], st["full_rows_read"], st["screen_kind"],
+                     st["screen_dims"]))
     ref[knob] = outs
-    print("screen=%s: %d checked batches in %.2f s" % (knob, pool, time.time() - t), flush=True)
-    if "used_after_search_gb" not in mem:
-        mem["used_after_search_gb"] = (total - torch.cuda.mem_get_info()[0]) / 1e9
-same = all(all(np.array_equal(a, b) for a, b in zip(o0[:3], o1[:3])) and o0[3:6] == o1[3:6] for o0, o1 in zip(ref["0"], ref["1"]))
-res = {"0": [], "1": []}
-kern = {"0": [], "1": []}
+    print("screen=%s: %d checked batches in %.2f s, kind %d, %d codes per candidate" % (knob, pool, time.time() - t, outs[0][7],
+                                                                                       outs[0][8]), flush=True)
+    mem["used_after_search_%s_gb" % knob] = (total - torch.cuda.mem_get_info()[0]) / 1e9
+same = all(all(np.array_equal(a, b) for a, b in zip(o0[:3], o1[:3])) and o0[3:6] == o1[3:6]
+           for kb in ref for o0, o1 in zip(ref[knobs[0]], ref[kb]))
+res = {kb: [] for kb in knobs}
+kern = {kb: [] for kb in knobs}
 for r in range(rounds):
-    for knob in ("0", "1"):
-        os.environ["LB200_SEARCH_SCREEN"] = knob
+    for knob in knobs:
+        if knob == "auto":
+            os.environ.pop("LB200_SEARCH_SCREEN", None)
+        else:
+            os.environ["LB200_SEARCH_SCREEN"] = knob
         for s in range(3):
             step(s)
         torch.cuda.synchronize()
@@ -75,18 +96,20 @@ for r in range(rounds):
             km += idx.last_stats()["kernel_ms"]
         kern[knob].append(km / 4)
         print("round %d screen=%s  %.0f queries/s  kernel %.2f ms/step" % (r, knob, res[knob][-1], kern[knob][-1]), flush=True)
-out = {"workload": wl_name, "identical_outputs_and_counters": bool(same), "memory": mem,
-       "gpu": torch.cuda.get_device_name(0)}
-for knob in ("0", "1"):
+out = {"workload": wl_name, "data": data, "identical_outputs_and_counters": bool(same), "memory": mem,
+       "gpu": torch.cuda.get_device_name(0), "auto_screen_kind": ref["auto"][0][7], "auto_screen_dims": ref["auto"][0][8]}
+for knob in knobs:
     v = np.array(res[knob])
     cd = sum(o[3] for o in ref[knob])
     fr = sum(o[6] for o in ref[knob])
     out["screen_" + knob] = {"qps_median": float(np.median(v)), "qps_min": float(v.min()), "qps_max": float(v.max()),
                              "kernel_ms_median": float(np.median(kern[knob])), "dist_evals_per_query": cd / (pool * B),
-                             "full_rows_read_per_query": fr / (pool * B), "full_rows_frac": fr / cd}
-out["speedup_median"] = out["screen_1"]["qps_median"] / out["screen_0"]["qps_median"]
+                             "full_rows_read_per_query": fr / (pool * B), "full_rows_frac": fr / cd,
+                             "screen_kind": ref[knob][0][7], "codes_per_candidate": ref[knob][0][8]}
+for knob in knobs[1:]:
+    out["speedup_median_%s_vs_%s" % (knob, knobs[0])] = out["screen_" + knob]["qps_median"] / out["screen_" + knobs[0]]["qps_median"]
 print(json.dumps(out))
 if os.environ.get("OUT"):  # directory for the JSON result
     os.makedirs(os.environ["OUT"], exist_ok=True)
-    with open(os.path.join(os.environ["OUT"], "exp_screen_%s.json" % wl_name), "w") as f:
+    with open(os.path.join(os.environ["OUT"], "exp_screen_%s_%s.json" % (wl_name, data)), "w") as f:
         json.dump(out, f, indent=1)
