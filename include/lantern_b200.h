@@ -118,6 +118,12 @@ typedef struct lb200_search_stats_t {
                                     screen of f32 l2sq / cos searches rejected from their codes alone */
     uint32_t screen_kind;        /* (appended field) the search's screen: 0 none, 1 int8 codes of every dimension, 2 projected codes */
     uint32_t screen_dims;        /* (appended field) codes per screened candidate: dimensions (1) or the basis' k (2) */
+    uint32_t search_kernel;      /* (appended field) the kernel that ran: 1 one CTA per query, 2 one warp per query */
+    uint32_t reserved;           /* (appended field) zero */
+    uint64_t owner_cycles_produce;  /* (appended fields) one warp per query: SM cycles of the walks' rounds by phase, summed */
+    uint64_t owner_cycles_screen;   /* over walks -- neighbour lists and visited bits, the projected screen, reading the   */
+    uint64_t owner_cycles_evaluate; /* surviving rows, the ordered insertions.  Zero for the CTA kernel.                    */
+    uint64_t owner_cycles_consume;
 } lb200_search_stats_t;
 
 /* Work of the most recent lb200_build (or implicit build): the build metric of SURVEY.md 8d is

@@ -56,7 +56,9 @@ class SearchStats(C.Structure):
     _fields_ = [("queries", C.c_uint64), ("computed_distances", C.c_uint64), ("base_pops", C.c_uint64),
                 ("upper_hops", C.c_uint64), ("algorithmic_bytes", C.c_uint64), ("kernel_ms", C.c_double),
                 ("limbo_overflows", C.c_uint64), ("full_rows_read", C.c_uint64), ("screen_kind", C.c_uint32),
-                ("screen_dims", C.c_uint32)]
+                ("screen_dims", C.c_uint32), ("search_kernel", C.c_uint32), ("reserved", C.c_uint32),
+                ("owner_cycles_produce", C.c_uint64), ("owner_cycles_screen", C.c_uint64), ("owner_cycles_evaluate", C.c_uint64),
+                ("owner_cycles_consume", C.c_uint64)]
 
 
 class BuildStats(C.Structure):

@@ -238,7 +238,7 @@ LB200_EXPORT void lb200_set_option(lb200_index_t h, char const* name, size_t val
             idx->build_ratio_ = value ? value : 1;
         else if (n == "search_expand")
             idx->search_expand_ = value ? value : 1;
-        else if (n == "search_kernel") { // 0 = by row width, 1 = one CTA per query, 2 = one warp per query
+        else if (n == "search_kernel") { // 0 / 1 = one CTA per query, 2 = one warp per query
             if (value > 2)
                 throw CudaError("search_kernel: 0, 1 or 2");
             idx->search_kernel_ = value;
@@ -328,6 +328,12 @@ LB200_EXPORT void lb200_last_search_stats(lb200_index_t h, lb200_search_stats_t*
         stats->full_rows_read = s.full_rows_read;
         stats->screen_kind = s.screen_kind;
         stats->screen_dims = s.screen_dims;
+        stats->search_kernel = s.search_kernel;
+        stats->reserved = 0;
+        stats->owner_cycles_produce = s.cycles_produce;
+        stats->owner_cycles_screen = s.cycles_screen;
+        stats->owner_cycles_evaluate = s.cycles_evaluate;
+        stats->owner_cycles_consume = s.cycles_consume;
     });
 }
 

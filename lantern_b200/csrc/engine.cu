@@ -16,9 +16,6 @@
 
 namespace lb200 {
 
-// rows up to this many bytes are searched by the warp-per-query kernel unless "search_kernel" says otherwise (0: never)
-constexpr size_t kWarpKernelMaxRowBytes = 0;
-
 std::atomic<uint64_t> g_kernel_launches{0};
 
 int device_sm_count() {
@@ -306,7 +303,9 @@ GraphView Index::view() const {
     g.sq_meta = d_sq_meta_;
     g.ps_records = reinterpret_cast<const uint4*>(d_ps_records_);
     g.ps_k = ps_k_;
-    g.flags = 2u; // L2-prefetch the adjacency line of nodes that enter the top list
+    // L2-prefetch the adjacency line of nodes that enter the top list (2); screened search rounds take both halves of a
+    // 64-wide list in one bitmap-atomic round trip (8)
+    g.flags = 2u | 8u;
     if (const char* e = getenv("LB200_FLAGS"))
         g.flags = (uint32_t)atoi(e);
     return g;
@@ -358,7 +357,7 @@ void Index::search_device(const void* d_queries, size_t nq, size_t stride, int k
         fill_results_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(d_keys, d_dists, d_counts, nq, k);
         LB_CUDA(cudaGetLastError());
         count_launch();
-        last_nq_ = 0;
+        last_nq_ = 0, last_kernel_ = 0;
         return;
     }
     size_t L = ef ? ef : cfg_.ef; // usearch.h:265-271: 0 = index default
@@ -372,18 +371,6 @@ void Index::search_device(const void* d_queries, size_t nq, size_t stride, int k
     launch_cast_rows(d_queries, stride, kind, qbuf, qrow, cfg_.pq ? (int)SK_F32 : cfg_.scalar_kind, cfg_.dims, nq, stream);
 
     const uint32_t expand = (uint32_t)std::min<size_t>(std::max<size_t>(search_expand_, 1), 8);
-    // kernel choice: one warp per query (no CTA barriers, more queries in flight) for narrow rows, one CTA per query with the
-    // bulk-copy ring for wide rows; "search_kernel" overrides
-    const bool warp_kernel = !cfg_.pq && expand == 1 && cfg_.M0 <= 256 &&
-                             (search_kernel_ == 2 || (search_kernel_ == 0 && row_bytes_ <= kWarpKernelMaxRowBytes));
-    if (warp_kernel) {
-        LB_CUDA(cudaEventRecord(ev0_, stream));
-        launch_warp_search(*this, qbuf, qrow, nq, k, (uint32_t)L, d_keys, d_dists, d_counts, stream);
-        LB_CUDA(cudaEventRecord(ev1_, stream));
-        last_nq_ = (uint32_t)nq;
-        last_screen_ = 0;
-        return;
-    }
     GraphView gv = view();
     if (cfg_.pq) {
         // the batch's look-up tables in one dense launch (49 KB per query at 96 x 128): the walk kernel then fetches a table with
@@ -429,6 +416,20 @@ void Index::search_device(const void* d_queries, size_t nq, size_t stride, int k
         launch_ps_queries(d_ps_basis_, d_ps_basis_t_, cfg_.dims, ps_k_, qbuf, qrow, nq, d_ps_query_, stream);
         gv.ps_query = d_ps_query_;
     }
+    // Kernel choice: one CTA per query unless "search_kernel" = 2.  One warp per query walks 24 queries per SM instead of 8 with
+    // no CTA barriers, and screens with the projected screen like the CTA kernel, but it measured slower even then (DESIGN.md
+    // 6: 0.90x at cfg3), so the automatic choice never takes it.
+    const bool warp_kernel = !cfg_.pq && expand == 1 && cfg_.M0 <= 256 && search_kernel_ == 2;
+    if (warp_kernel) {
+        LB_CUDA(cudaEventRecord(ev0_, stream));
+        launch_warp_search(*this, qbuf, qrow, nq, k, (uint32_t)L, screen == 2 ? d_ps_query_ : nullptr, d_keys, d_dists, d_counts,
+                           stream);
+        LB_CUDA(cudaEventRecord(ev1_, stream));
+        last_nq_ = (uint32_t)nq;
+        last_screen_ = screen == 2 ? 2 : 0;
+        last_kernel_ = 2;
+        return;
+    }
     const uint32_t max_ctas = search_max_ctas(dist_mode_, cfg_.scalar_kind, gv, (uint32_t)L, cfg_.pq, expand, screen);
     ensure_scratch(max_ctas);
     LB_CUDA(cudaMemsetAsync(scratch_.counters, 0, 8 * sizeof(unsigned long long), stream));
@@ -448,6 +449,7 @@ void Index::search_device(const void* d_queries, size_t nq, size_t stride, int k
     LB_CUDA(cudaEventRecord(ev1_, stream));
     last_nq_ = (uint32_t)nq;
     last_screen_ = screen;
+    last_kernel_ = 1;
 }
 
 void Index::search_host(const void* queries, size_t nq, size_t stride, int kind, size_t k, size_t ef, uint64_t* keys,
@@ -489,8 +491,16 @@ SearchStats Index::last_stats() {
     std::lock_guard<std::mutex> g(mu_);
     unsigned long long c[8] = {0};
     LB_CUDA(cudaDeviceSynchronize());
-    LB_CUDA(cudaMemcpy(c, scratch_.counters, sizeof(c), cudaMemcpyDeviceToHost));
     SearchStats s;
+    if (last_kernel_ == 2) { // the warp kernel's counters (GroupLaunch::counters) in the search's order
+        unsigned long long w[16] = {0};
+        LB_CUDA(cudaMemcpy(w, d_warp_aux_, sizeof(w), cudaMemcpyDeviceToHost));
+        c[1] = w[1], c[2] = w[2], c[3] = w[3], c[4] = w[7], c[5] = w[12], c[6] = w[13];
+        s.cycles_produce = w[8], s.cycles_screen = w[14], s.cycles_evaluate = w[9] + w[10], s.cycles_consume = w[11];
+    } else {
+        LB_CUDA(cudaMemcpy(c, scratch_.counters, sizeof(c), cudaMemcpyDeviceToHost));
+    }
+    s.search_kernel = (uint32_t)last_kernel_;
     s.queries = last_nq_;
     if (last_nq_) {
         float ms = 0.f;

@@ -43,6 +43,9 @@ struct SearchStats {
     uint32_t screen_kind = 0;    // 0 = no screen, 1 = int8 codes, 2 = projected codes
     uint32_t screen_dims = 0;    // codes per screened candidate: dims (int8) or k (projected)
     double kernel_ms = 0; // device time of the search kernel alone (CUDA events on the launching stream)
+    uint32_t search_kernel = 0;  // 1 = one CTA per query (search.cu), 2 = one warp per query (group.cu)
+    // one warp per query: SM cycles of the walks' rounds, summed over walks (zero for the CTA kernel)
+    uint64_t cycles_produce = 0, cycles_screen = 0, cycles_evaluate = 0, cycles_consume = 0;
 };
 
 // Device-side view handed to kernels (plain pointers, trivially copyable).
@@ -62,7 +65,8 @@ struct GraphView {
     const float* pq_pair;  // [nsub][ncent][ncent] centroid-pair table (l2sq: |ca-cb|^2 ; cos: ca.cb)
     const float* pq_norm;  // [nsub][ncent] |centroid slice|^2 (cos)
     const float* pq_query_tables; // search only: per-query look-up tables [nq][pq_table_floats] precomputed for the batch, or NULL
-    uint32_t flags;        // tuning: 1 = L2-prefetch the adjacency of every measured node, 2 = of accepted nodes only
+    uint32_t flags;        // tuning: 1 = L2-prefetch the adjacency of every measured node, 2 = of accepted nodes only;
+                           // 8 = screened search rounds visit a 64-wide list in one bitmap-atomic round trip
     uint32_t dims, num_centroids, num_subvectors;
     uint32_t pq_lut_width; // centroids the per-value table covers (= num_centroids, or 128 when every stored code is < 128)
     // search screen (f32 l2sq / cos): int8 code rows of screen_code_bytes(row_bytes) and their metadata, or NULL
@@ -160,7 +164,7 @@ class Index {
     size_t build_ratio_ = 64;   // a batch never exceeds (visible nodes) / build_ratio_
     uint32_t touched_cap_ = 16384; // per-CTA log of bitmap words to un-visit; beyond it the whole bitmap is cleared
     size_t search_expand_ = 1;  // 1 = exact-order search; 2..4 = relaxed order (see walk.cuh)
-    size_t search_kernel_ = 0;  // 0 = pick by row width, 1 = one CTA per query (search.cu), 2 = one warp per query (group.cu)
+    size_t search_kernel_ = 0;  // 0 / 1 = one CTA per query (search.cu), 2 = one warp per query (group.cu)
     bool pq_query_tables_ = true; // pq search: precompute the batch's look-up tables when they fit in 1 GB; false = never
     uint8_t* d_warp_aux_ = nullptr; // warp kernel: counters, flags, dummy counts
     size_t warp_aux_bytes_ = 0;
@@ -199,6 +203,7 @@ class Index {
     bool ps_auto_ = false;     // ... and it is the projected screen (a basis may also exist because LB200_SEARCH_SCREEN=2 forced one)
     double ps_basis_ms_ = 0;   // host time of the last basis choice (moment matrix, eigenvectors, records)
     int last_screen_ = 0;      // screen kind of the last search
+    int last_kernel_ = 0;      // search kernel of the last search: 1 = one CTA per query, 2 = one warp per query
     size_t pending_raw_cap_ = 0;
     // host mirrors of the small per-node metadata
     std::vector<int16_t> h_levels_;
@@ -295,9 +300,10 @@ void launch_search(int dist_mode, int scalar_kind, bool pq, const SearchLaunch& 
 // (every stored row, measured cand_cap at a time) and d_lut[count][nsub * pq_lut_width + 1] (the table, then |value|^2).
 void launch_pq_probe(int dist_mode, const GraphView& g, uint32_t cand_cap, const uint8_t* d_values, uint32_t value_stride,
                      const uint32_t* d_nodes, size_t count, float* d_dist, float* d_lut, cudaStream_t stream);
-// group.cu: the warp-per-query kernel as a single-GPU search path
-void launch_warp_search(Index& idx, const uint8_t* qbuf, size_t qrow, size_t nq, size_t k, uint32_t L, uint64_t* d_keys, float* d_dists,
-                        uint32_t* d_counts, cudaStream_t stream);
+// group.cu: the warp-per-query kernel as a single-GPU search path; ps_query = the batch's projected-screen pre-pass (the
+// level-0 rounds screen their candidates), or NULL (no screen).  Work counters land in idx.d_warp_aux_ (Index::last_stats).
+void launch_warp_search(Index& idx, const uint8_t* qbuf, size_t qrow, size_t nq, size_t k, uint32_t L, const float* ps_query,
+                        uint64_t* d_keys, float* d_dists, uint32_t* d_counts, cudaStream_t stream);
 // exact_tc.cu: launch plan of the tensor-core filter, and a test hook that copies its intermediate buffers to the host
 struct ExactTcEps { // |approximate - exact fp32 distance| <= eps(|q|^2, |x|^2): see approx_eps in exact_tc.cu
     float rel;       // 3xTF32 dot product, relative to |q||x|

@@ -78,10 +78,12 @@ __device__ __forceinline__ uint4 ld_nocache_u4(const uint4* p) {
 }
 
 struct GroupWarpLayout {
-    uint32_t ring, bars, top_d, top_i, cand_id, cand_d, cand_slot, loc, limbo, total;
+    uint32_t ring, bars, top_d, top_i, cand_id, cand_d, cand_slot, loc, limbo, psq, total;
 };
-// per warp: R row slots (the bulk-copy ring), R mbarriers, the top list, the candidate arrays
-__host__ __device__ inline GroupWarpLayout group_warp_layout(uint32_t row_bytes, uint32_t R, uint32_t L, uint32_t cap) {
+// per warp: R row slots (the bulk-copy ring), R mbarriers, the top list, the candidate arrays, and for the projected screen
+// the query's q~ and its header (psq_floats = ps_query_floats(k); 0 without the screen)
+__host__ __device__ inline GroupWarpLayout group_warp_layout(uint32_t row_bytes, uint32_t R, uint32_t L, uint32_t cap,
+                                                             uint32_t psq_floats = 0) {
     GroupWarpLayout l;
     uint32_t o = 0;
     l.ring = o, o += R * ((row_bytes + 15u) & ~15u);
@@ -93,6 +95,8 @@ __host__ __device__ inline GroupWarpLayout group_warp_layout(uint32_t row_bytes,
     l.cand_slot = o, o += (2 * cap + 3u) & ~3u;
     l.loc = o, o += (cap + 3u) & ~3u;
     l.limbo = o, o += 4 * kLimboCap;
+    o = (o + 15u) & ~15u;
+    l.psq = o, o += 4 * psq_floats;
     l.total = (o + 15u) & ~15u;
     return l;
 }
@@ -115,7 +119,8 @@ constexpr uint32_t kMsgExit = 0xFFFFFFFFu;
 constexpr uint32_t kMsgCountBits = 9;
 constexpr size_t kGroupMaxBatch = (size_t)1 << (32 - kMsgCountBits - 1);
 
-template <int DM, int SK, int NQ> struct GroupWarp {
+// PS: the level-0 rounds of the owner run the projected screen (screen.cuh) -- one rank only, f32 l2sq / cos
+template <int DM, int SK, int NQ, bool PS = false> struct GroupWarp {
     const GroupLaunch& p;
     int lane;
     uint32_t slot, nchunks;
@@ -131,11 +136,15 @@ template <int DM, int SK, int NQ> struct GroupWarp {
     uint32_t st_dist, st_pops, st_hops, st_rounds, st_rows;
     // owner: SM cycles spent producing a round's ids, measuring the local rows, waiting for the helpers, consuming
     uint32_t cy_produce, cy_local, cy_wait, cy_consume; // (32 bits: 2 s of cycles per warp and launch)
+    uint32_t cy_screen, st_screened, st_rejected;       // PS only
 
     __device__ __forceinline__ explicit GroupWarp(const GroupLaunch& gp) : p(gp) {}
 
+    __device__ __forceinline__ uint32_t psq_floats() const { return PS ? ps_query_floats(p.g.ps_k) : 0u; }
     // shared-memory arrays are addressed from one base (fewer live registers than eight pointers)
-    __device__ __forceinline__ GroupWarpLayout lay() const { return group_warp_layout(p.g.row_bytes, p.ring_slots, p.L, p.cap); }
+    __device__ __forceinline__ GroupWarpLayout lay() const {
+        return group_warp_layout(p.g.row_bytes, p.ring_slots, p.L, p.cap, psq_floats());
+    }
     __device__ __forceinline__ uint8_t* ring() const { return ws; }
     __device__ __forceinline__ uint64_t* bars() const { return reinterpret_cast<uint64_t*>(ws + lay().bars); }
     __device__ __forceinline__ float* top_d() const { return reinterpret_cast<float*>(ws + lay().top_d); }
@@ -145,6 +154,7 @@ template <int DM, int SK, int NQ> struct GroupWarp {
     __device__ __forceinline__ uint16_t* cand_slot() const { return reinterpret_cast<uint16_t*>(ws + lay().cand_slot); }
     __device__ __forceinline__ uint8_t* loc() const { return ws + lay().loc; }
     __device__ __forceinline__ uint32_t* limbo() const { return reinterpret_cast<uint32_t*>(ws + lay().limbo); }
+    __device__ __forceinline__ float* psq() const { return reinterpret_cast<float*>(ws + lay().psq); }
 
     __device__ __noinline__ bool timed_out() {
         if (ld_sys_u32(p.err[p.me]) != 0u)
@@ -416,6 +426,76 @@ template <int DM, int SK, int NQ> struct GroupWarp {
         }
     }
 
+    // ---- owner, PS: the projected screen of a level-0 round (PScreenEval::screen on one warp).  Lane l takes candidates
+    // l, l + 32, ...: two 64-byte records per lane travel together (one round trip for a 64-wide list), 128-byte ones one at a
+    // time; the bound is pscreen_bound on ps_accum's sums, as in the CTA kernel.  cand_id[0..n) -> the candidates with
+    // !(lb >= radius), compacted in stored order; returns their number.  Not inlined: the bound's double arithmetic then
+    // lives in its own frame instead of adding to the walk's spills at the 80-register cap of 6 CTAs/SM.
+    __device__ __forceinline__ float pscreen_lb(const uint4 (&v)[8], bool wide, float4 qh, uint32_t slots) const {
+        const float* qt = psq();
+        float sf = 0.f, cc = 0.f;
+        ps_accum(qt, v[1], sf, cc);
+        ps_accum(qt + 16, v[2], sf, cc);
+        ps_accum(qt + 32, v[3], sf, cc);
+        if (wide) {
+            ps_accum(qt + 48, v[4], sf, cc);
+            ps_accum(qt + 64, v[5], sf, cc);
+            ps_accum(qt + 80, v[6], sf, cc);
+            ps_accum(qt + 96, v[7], sf, cc);
+        }
+        const float4 meta = make_float4(__uint_as_float(v[0].x), __uint_as_float(v[0].y), __uint_as_float(v[0].z), __uint_as_float(v[0].w));
+        return pscreen_bound<DM, NQ>(sf, cc, meta, qh, a2, slots);
+    }
+    __device__ __noinline__ uint32_t pscreen(uint32_t n, float radius) {
+        const uint32_t slots = ps_code_slots(p.g.ps_k), rec = ps_record_bytes(p.g.ps_k) / 16;
+        const float4 qh = *reinterpret_cast<const float4*>(psq() + slots);
+        uint32_t* ids = cand_id();
+        float* lbs = cand_d();
+#pragma unroll 1
+        for (uint32_t j = lane; j < n; j += 64) {
+            uint4 a[8], b[8];
+            const uint4* ra = p.g.ps_records + (size_t)ids[j] * rec;
+            if (rec == 4) {
+                const bool two = j + 32 < n;
+                const uint4* rb = p.g.ps_records + (size_t)ids[two ? j + 32 : j] * rec;
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+                    a[i] = __ldg(ra + i), b[i] = __ldg(rb + i);
+                lbs[j] = pscreen_lb(a, false, qh, slots);
+                if (two)
+                    lbs[j + 32] = pscreen_lb(b, false, qh, slots);
+            } else {
+#pragma unroll
+                for (int i = 0; i < 8; ++i)
+                    a[i] = __ldg(ra + i);
+                lbs[j] = pscreen_lb(a, true, qh, slots);
+                if (j + 32 < n) {
+                    const uint4* rb = p.g.ps_records + (size_t)ids[j + 32] * rec;
+#pragma unroll
+                    for (int i = 0; i < 8; ++i)
+                        b[i] = __ldg(rb + i);
+                    lbs[j + 32] = pscreen_lb(b, true, qh, slots);
+                }
+            }
+        }
+        __syncwarp();
+        const uint32_t lt = (1u << lane) - 1u;
+        uint32_t m = 0;
+        for (uint32_t base = 0; base < n; base += 32) {
+            const uint32_t j = base + lane;
+            const bool keep = j < n && !(lbs[j] >= radius);
+            const uint32_t id = j < n ? ids[j] : 0u;
+            const uint32_t mk = __ballot_sync(0xffffffffu, keep);
+            __syncwarp();
+            if (keep)
+                ids[m + __popc(mk & lt)] = id;
+            m += __popc(mk);
+        }
+        __syncwarp();
+        st_screened += n, st_rejected += n - m;
+        return m;
+    }
+
     __device__ __forceinline__ void tell_helpers(uint32_t payload) {
         const uint32_t flag = p.flag_base + (++seq);
         if ((uint32_t)lane < p.G && (uint32_t)lane != p.me)
@@ -431,6 +511,13 @@ template <int DM, int SK, int NQ> struct GroupWarp {
         uint32_t* touched = p.touched + (size_t)slot * p.touched_cap;
         load_query(q);
         cur_q = q;
+        if constexpr (PS) { // q~ and its header from the batch's pre-pass (launch_ps_queries)
+            const uint32_t nf = psq_floats();
+            __syncwarp(); // the previous query's screen is done with psq
+            for (uint32_t i = lane; i < nf; i += 32)
+                psq()[i] = __ldg(p.g.ps_query + (size_t)q * nf + i);
+            __syncwarp();
+        }
         if (p.G > 1) { // the helpers read the query from the mailbox of this owner slot on THEIR GPU
             for (uint32_t d = 0; d < p.G; ++d) {
                 if (d == p.me)
@@ -566,6 +653,16 @@ template <int DM, int SK, int NQ> struct GroupWarp {
             }
             __syncwarp();
             const uint32_t cp1 = (uint32_t)clock64();
+            const uint32_t n_all = n; // the screen's rejects count as computed distances: the reference computes them
+            if constexpr (PS) {
+                // a level-0 round that starts with a full top list: a candidate can enter only below td[L-1], and the radius
+                // only shrinks within the round, so screening against its start is safe (WalkerT::beam_impl's rule, which
+                // also skips a NaN radius)
+                const float radius = level == 0 && size == L ? top_d()[size - 1] : __int_as_float(0x7fffffff);
+                if (radius == radius && n)
+                    n = pscreen(n, radius);
+                cy_screen += (uint32_t)clock64() - cp1;
+            }
             // ---- evaluate: every id on the GPU that holds its row ----
             if (n)
                 eval_round(n);
@@ -573,7 +670,7 @@ template <int DM, int SK, int NQ> struct GroupWarp {
                 break;
             const uint32_t cp2 = (uint32_t)clock64();
             cy_produce += cp1 - cp0; // classification + sends are counted with the evaluation
-            st_dist += n;
+            st_dist += n_all;
             // ---- consume ----
             if (level < 0) {
                 cur_d = cand_d()[0];
@@ -669,15 +766,15 @@ template <int DM, int SK, int NQ> struct GroupWarp {
     }
 };
 
-template <int DM, int SK, int NQ>
+template <int DM, int SK, int NQ, bool PS = false>
 __global__ void __launch_bounds__(kGroupThreads, 6) group_search_kernel(const __grid_constant__ GroupLaunch p) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
-    GroupWarp<DM, SK, NQ> w(p);
+    GroupWarp<DM, SK, NQ, PS> w(p);
     w.lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
     w.slot = blockIdx.x * kGroupWarps + warp;
     w.nchunks = p.g.row_bytes / 16;
-    w.ws = smem_raw + (size_t)warp * group_warp_layout(p.g.row_bytes, p.ring_slots, p.L, p.cap).total;
+    w.ws = smem_raw + (size_t)warp * w.lay().total;
     w.phase_bits = 0;
     if (w.lane == 0) {
         for (uint32_t i = 0; i < p.ring_slots; ++i)
@@ -689,6 +786,7 @@ __global__ void __launch_bounds__(kGroupThreads, 6) group_search_kernel(const __
     w.waited = (p.me == p.root);
     w.st_dist = w.st_pops = w.st_hops = w.st_rounds = w.st_rows = 0;
     w.cy_produce = w.cy_local = w.cy_wait = w.cy_consume = 0;
+    w.cy_screen = w.st_screened = w.st_rejected = 0;
     w.t0 = globaltimer_ns();
 
     // the root's query staging buffer is complete when its kernel starts (stream order): tell everybody
@@ -725,6 +823,10 @@ __global__ void __launch_bounds__(kGroupThreads, 6) group_search_kernel(const __
             atomicAdd(&p.counters[8], (unsigned long long)w.cy_produce), atomicAdd(&p.counters[9], (unsigned long long)w.cy_local);
             atomicAdd(&p.counters[10], (unsigned long long)w.cy_wait), atomicAdd(&p.counters[11], (unsigned long long)w.cy_consume);
         }
+        if constexpr (PS) {
+            atomicAdd(&p.counters[12], (unsigned long long)w.st_screened), atomicAdd(&p.counters[13], (unsigned long long)w.st_rejected);
+            atomicAdd(&p.counters[14], (unsigned long long)w.cy_screen);
+        }
         __threadfence();
         last_warp = atomicAdd(&p.counters[0], 1ull) == (unsigned long long)gridDim.x * kGroupWarps - 1ull;
     }
@@ -744,15 +846,15 @@ __global__ void __launch_bounds__(kGroupThreads, 6) group_search_kernel(const __
     }
 }
 
-template <int DM, int SK, int NQ> void group_launch_one(const GroupLaunch& p, uint32_t grid, size_t smem, cudaStream_t stream) {
-    auto kern = group_search_kernel<DM, SK, NQ>;
+template <int DM, int SK, int NQ, bool PS = false> void group_launch_one(const GroupLaunch& p, uint32_t grid, size_t smem, cudaStream_t stream) {
+    auto kern = group_search_kernel<DM, SK, NQ, PS>;
     LB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kern<<<grid, kGroupThreads, smem, stream>>>(p);
     LB_CUDA(cudaGetLastError());
     count_launch();
 }
-template <int DM, int SK, int NQ> int group_occupancy_one(size_t smem) {
-    auto kern = group_search_kernel<DM, SK, NQ>;
+template <int DM, int SK, int NQ, bool PS = false> int group_occupancy_one(size_t smem) {
+    auto kern = group_search_kernel<DM, SK, NQ, PS>;
     LB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int blocks = 0;
     LB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, kGroupThreads, smem));
@@ -1574,19 +1676,33 @@ Group* group_create_local(const int* devices, int ndev) {
 // One warp per query instead of one CTA per query (search.cu): no CTA-wide barriers, 28 queries in flight per SM instead of
 // 8-10.  For narrow rows (binary vectors, short f16/i8 rows) the per-expansion serial chain of the CTA kernel -- warp 0
 // working while three warps wait at the barrier -- is what bounds it; here every warp always has its own work.
-void launch_warp_search(Index& idx, const uint8_t* qbuf, size_t qrow, size_t nq, size_t k, uint32_t L, uint64_t* d_keys, float* d_dists,
-                        uint32_t* d_counts, cudaStream_t stream) {
+// fn(dm, sk, nq, ps) tags of the warp kernel: ps = std::true_type for the projected-screen owner (f32 l2sq / cos only)
+template <typename Fn> static void dispatch_warp_kernel(int dm, int sk, int nq, bool ps, Fn&& fn) {
+    dispatch_walk(dm, sk, nq, [&](auto d, auto s, auto q) {
+        if (!ps)
+            return fn(d, s, q, std::false_type{});
+        if constexpr (decltype(s)::value == SK_F32 && (decltype(d)::value == DM_L2SQ || decltype(d)::value == DM_COS))
+            fn(d, s, q, std::true_type{});
+        else
+            throw CudaError("warp search: the projected screen needs f32 l2sq / cos rows");
+    });
+}
+
+void launch_warp_search(Index& idx, const uint8_t* qbuf, size_t qrow, size_t nq, size_t k, uint32_t L, const float* ps_query,
+                        uint64_t* d_keys, float* d_dists, uint32_t* d_counts, cudaStream_t stream) {
     const IndexConfig& cfg = idx.cfg_;
     if (cfg.pq)
         throw CudaError("warp search: pq indexes use the CTA kernel");
     const uint32_t cap = (uint32_t)cfg.M0;
     if (cap > 256)
         throw CudaError("warp search: connectivity above 128 is not supported");
+    const bool ps = ps_query != nullptr;
     const int nqc = pick_nq((uint32_t)idx.row_bytes_);
-    const size_t smem = (size_t)group_warp_layout((uint32_t)idx.row_bytes_, group_ring_slots((uint32_t)idx.row_bytes_), L, cap).total * kGroupWarps;
+    const size_t smem = (size_t)group_warp_layout((uint32_t)idx.row_bytes_, group_ring_slots((uint32_t)idx.row_bytes_), L, cap,
+                                                  ps ? ps_query_floats(idx.ps_k_) : 0u).total * kGroupWarps;
     int occ = 0;
-    dispatch_walk(idx.dist_mode_, cfg.scalar_kind, nqc, [&](auto d, auto s2, auto q) {
-        occ = group_occupancy_one<decltype(d)::value, decltype(s2)::value, decltype(q)::value>(smem);
+    dispatch_warp_kernel(idx.dist_mode_, cfg.scalar_kind, nqc, ps, [&](auto d, auto s2, auto q, auto sc) {
+        occ = group_occupancy_one<decltype(d)::value, decltype(s2)::value, decltype(q)::value, decltype(sc)::value>(smem);
     });
     if (occ < 1)
         throw CudaError("warp search: kernel does not fit on an SM (ef too large for shared memory)");
@@ -1609,6 +1725,7 @@ void launch_warp_search(Index& idx, const uint8_t* qbuf, size_t qrow, size_t nq,
     p.flag_base = 1u << 20, p.epoch = 1, p.root = 0;
     p.timeout_ns = ~0ull;
     p.g = idx.view();
+    p.g.ps_query = ps_query;
     p.bounds[0] = 0;
     for (int r = 1; r <= kGroupMax; ++r)
         p.bounds[r] = 0xFFFFFFFFu;
@@ -1619,14 +1736,15 @@ void launch_warp_search(Index& idx, const uint8_t* qbuf, size_t qrow, size_t nq,
     p.queries = qbuf, p.query_stride = (uint32_t)qrow;
     p.vis = idx.scratch_.visited, p.touched = idx.scratch_.touched;
     p.words_per_slot = idx.scratch_.words_per_cta, p.touched_cap = idx.scratch_.touched_cap;
-    p.O = (uint32_t)std::min<size_t>(W & ~3u, round_up(nq, kGroupWarps)), p.H = 0;
+    // equal waves: ceil(nq / ceil(nq / W)) owners rather than min(W, nq) -- at 4096 queries and W = 3168, 2048 walks of 2
+    // queries each instead of 3168 walks whose second wave is mostly idle (measured 8 % faster at cfg3, DESIGN.md 6)
+    const size_t waves = (nq + (W & ~3u) - 1) / (W & ~3u);
+    p.O = (uint32_t)std::min<size_t>(W & ~3u, round_up((nq + waves - 1) / waves, kGroupWarps)), p.H = 0;
     const uint32_t grid = p.O / kGroupWarps;
-    dispatch_walk(idx.dist_mode_, cfg.scalar_kind, nqc, [&](auto d, auto s2, auto q) {
-        group_launch_one<decltype(d)::value, decltype(s2)::value, decltype(q)::value>(p, grid, smem, stream);
+    dispatch_warp_kernel(idx.dist_mode_, cfg.scalar_kind, nqc, ps, [&](auto d, auto s2, auto q, auto sc) {
+        group_launch_one<decltype(d)::value, decltype(s2)::value, decltype(q)::value, decltype(sc)::value>(p, grid, smem, stream);
     });
-    // work counters where Index::last_stats() reads them: [1] distance evaluations, [2] base pops, [3] upper hops
-    LB_CUDA(cudaMemcpyAsync(idx.scratch_.counters + 1, p.counters + 1, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, stream));
-    LB_CUDA(cudaMemcpyAsync(idx.scratch_.counters + 4, p.counters + 7, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, stream));
+    // Index::last_stats() reads p.counters (d_warp_aux_) after a warp search
 }
 
 void group_free(Group* G) {

@@ -811,6 +811,56 @@ template <class E> struct WalkerT : E {
                         continue;
                     uint32_t width;
                     const uint32_t* list = list_of(c, level, width);
+                    bool halves = false; // screened search walkers only: builds and unscreened searches keep the loop below
+                    if constexpr (E::kScreen)
+                        halves = width == 64 && n == 0 && (g.flags & 8u);
+                    if (halves) {
+                        // both halves of a 64-wide list at once (flags bit 8): the two bitmap atomics of a lane are in flight
+                        // together, one L2 round trip instead of two.  Only the FIRST occurrence of an id in stored order may
+                        // count as unseen, so the second half is also checked against the first (through cand_id, free here:
+                        // n == 0).  The same selection and order as the loop below (group.cu's owner does the same).
+                        const uint32_t id0 = __ldg(list + lane), id1 = __ldg(list + 32 + lane);
+                        const bool v0 = id0 != kNoNeighbor, v1 = id1 != kNoNeighbor;
+                        sm.cand_id[lane] = id0;
+                        __syncwarp();
+                        const uint32_t p0 = __match_any_sync(0xffffffffu, id0), p1 = __match_any_sync(0xffffffffu, id1);
+                        const bool first0 = v0 && ((uint32_t)(__ffs(p0) - 1) == (uint32_t)lane);
+                        bool first1 = v1 && ((uint32_t)(__ffs(p1) - 1) == (uint32_t)lane);
+                        if (first1)
+                            for (int t = 0; t < 32; ++t)
+                                first1 &= sm.cand_id[t] != id1;
+                        __syncwarp();
+                        const uint32_t bit0 = 1u << (id0 & 31), bit1 = 1u << (id1 & 31);
+                        uint32_t old0 = 0, old1 = 0;
+                        if (first0)
+                            old0 = atomicOr(&vis[id0 >> 5], bit0);
+                        if (first1)
+                            old1 = atomicOr(&vis[id1 >> 5], bit1);
+                        const bool fresh0 = first0 && !(old0 & bit0), fresh1 = first1 && !(old1 & bit1);
+                        const uint32_t m0 = __ballot_sync(0xffffffffu, fresh0), m1 = __ballot_sync(0xffffffffu, fresh1);
+                        const uint32_t lt = (1u << lane) - 1u, n0 = __popc(m0);
+                        if (fresh0) {
+                            const uint32_t r = __popc(m0 & lt);
+                            sm.cand_id[r] = id0;
+                            if (ntouched + r < touched_cap)
+                                touched[ntouched + r] = id0 >> 5;
+                            if (level == 0 && (g.flags & 1u))
+                                prefetch_l2(g.adj0 + (size_t)id0 * g.M0);
+                        }
+                        __syncwarp(); // the compaction above overwrites entries another lane compared against
+                        if (fresh1) {
+                            const uint32_t r = n0 + __popc(m1 & lt);
+                            sm.cand_id[r] = id1;
+                            if (ntouched + r < touched_cap)
+                                touched[ntouched + r] = id1 >> 5;
+                            if (level == 0 && (g.flags & 1u))
+                                prefetch_l2(g.adj0 + (size_t)id1 * g.M0);
+                        }
+                        n = n0 + __popc(m1);
+                        ntouched += n;
+                        st_pops += 1;
+                        continue;
+                    }
                     for (uint32_t off = 0; off < width; off += 32) {
                         uint32_t id = (off + lane < width) ? __ldg(list + off + lane) : kNoNeighbor;
                         bool valid = id != kNoNeighbor;

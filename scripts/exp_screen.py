@@ -1,14 +1,16 @@
-"""Dev experiment: the search screens (LB200_SEARCH_SCREEN 0 = off, 1 = int8, 2 = projected) on ONE built graph (needs a GPU).
+"""Dev experiment: the search screens (LB200_SEARCH_SCREEN 0 = off, 1 = int8, 2 = projected) and search kernels on ONE built
+graph (needs a GPU).
 
 Builds a workload's graph once with bench.py's generator and seeds (DATA=gauss: isotropic Gaussian rows and queries instead),
-then alternates the knobs for ROUNDS rounds of STEPS timed search steps each.  Prints, per setting, queries/s (median and
-spread over the rounds), kernel time, the share of candidates read in full (full_rows_read / computed_distances), the screen
-kind and codes per candidate, that every setting returns identical keys, distances and counters, and the device memory in use
-after the build (with the automatically chosen companion) and after each setting's first search (a forced kind encodes its
-companion then).
+then alternates every (kernel, knob) setting for ROUNDS rounds of STEPS timed search steps each.  Prints, per setting,
+queries/s (median and spread over the rounds), kernel time, the share of candidates read in full (full_rows_read /
+computed_distances), the screen kind and codes per candidate, the kernel that ran and its cycle split by phase (one warp per
+query), that every setting returns identical keys, distances and counters, and the device memory in use after the build (with
+the automatically chosen companion) and after each setting's first search (a forced kind encodes its companion then).
 usage: python scripts/exp_screen.py [workload] ; env ROUNDS (default 3), STEPS (default 20), KNOBS (default 0,1,2; "auto" =
-unset),
-DATA (structured | gauss), OUT (directory for the JSON)"""
+unset), KERNELS (default "0": the "search_kernel" option, 0 = automatic, 1 = one CTA per query, 2 = one warp per query;
+"1w2" = one CTA of 2 warps per query with 12 KB rings, LB200_SEARCH_WARPS=2 LB200_RING_BYTES=12288), DATA (structured |
+gauss), OUT (directory for the JSON)"""
 import json, os, sys, time
 sys.path.insert(0, '.')
 import numpy as np, torch
@@ -19,6 +21,8 @@ wl_name = sys.argv[1] if len(sys.argv) > 1 else "cfg3"
 wl = bench.WORKLOADS[wl_name]
 rounds, steps = int(os.environ.get("ROUNDS", "3")), int(os.environ.get("STEPS", "20"))
 knobs = os.environ.get("KNOBS", "0,1,2").split(",")
+kernels = os.environ.get("KERNELS", "0").split(",")
+settings = [(kn, kb) for kn in kernels for kb in knobs]
 data = os.environ.get("DATA", "structured")
 n, dim, B, k, ef = wl["n"], wl["dim"], wl["batch"], wl["k"], wl["ef"]
 dev = torch.device("cuda", 0)
@@ -53,13 +57,25 @@ def step(s):
                             stream.cuda_stream)
 
 
-ref = {}
-for knob in ["auto"] + knobs:  # outputs and counters of every pool batch, every way
-    if knob == "auto":
-        os.environ.pop("LB200_SEARCH_SCREEN", None)
-    else:
+def apply(kern, knob):
+    for var in ("LB200_SEARCH_SCREEN", "LB200_SEARCH_WARPS", "LB200_RING_BYTES"):
+        os.environ.pop(var, None)
+    if knob != "auto":
         os.environ["LB200_SEARCH_SCREEN"] = knob
-    outs = []
+    if kern == "1w2":
+        os.environ["LB200_SEARCH_WARPS"], os.environ["LB200_RING_BYTES"] = "2", "12288"
+    idx.set_option("search_kernel", 1 if kern == "1w2" else int(kern))
+
+
+def name(kern, knob):
+    return "screen=%s" % knob if kernels == ["0"] else "kernel=%s,screen=%s" % (kern, knob)
+
+
+CYCLES = ("owner_cycles_produce", "owner_cycles_screen", "owner_cycles_evaluate", "owner_cycles_consume")
+ref, cyc = {}, {}
+for kern, knob in [("0", "auto")] + settings:  # outputs and counters of every pool batch, every way
+    apply(kern, knob)
+    outs, cy = [], np.zeros(len(CYCLES))
     t = time.time()
     for s in range(pool):
         step(s)
@@ -67,21 +83,20 @@ for knob in ["auto"] + knobs:  # outputs and counters of every pool batch, every
         st = idx.last_stats()
         outs.append((ok.cpu().numpy().copy(), od.cpu().numpy().view(np.uint32).copy(), oc.cpu().numpy().copy(),
                      st["computed_distances"], st["base_pops"], st["upper_hops"], st["full_rows_read"], st["screen_kind"],
-                     st["screen_dims"]))
-    ref[knob] = outs
-    print("screen=%s: %d checked batches in %.2f s, kind %d, %d codes per candidate" % (knob, pool, time.time() - t, outs[0][7],
-                                                                                       outs[0][8]), flush=True)
-    mem["used_after_search_%s_gb" % knob] = (total - torch.cuda.mem_get_info()[0]) / 1e9
+                     st["screen_dims"], st["search_kernel"]))
+        cy += [st[c] for c in CYCLES]
+    ref[name(kern, knob)], cyc[name(kern, knob)] = outs, cy
+    print("%s: %d checked batches in %.2f s, kind %d, %d codes per candidate, kernel %d" % (
+        name(kern, knob), pool, time.time() - t, outs[0][7], outs[0][8], outs[0][9]), flush=True)
+    mem["used_after_search_%s_gb" % name(kern, knob)] = (total - torch.cuda.mem_get_info()[0]) / 1e9
+names = [name(kn, kb) for kn, kb in settings]
 same = all(all(np.array_equal(a, b) for a, b in zip(o0[:3], o1[:3])) and o0[3:6] == o1[3:6]
-           for kb in ref for o0, o1 in zip(ref[knobs[0]], ref[kb]))
-res = {kb: [] for kb in knobs}
-kern = {kb: [] for kb in knobs}
+           for kb in ref for o0, o1 in zip(ref[names[0]], ref[kb]))
+res = {nm: [] for nm in names}
+kern_ms = {nm: [] for nm in names}
 for r in range(rounds):
-    for knob in knobs:
-        if knob == "auto":
-            os.environ.pop("LB200_SEARCH_SCREEN", None)
-        else:
-            os.environ["LB200_SEARCH_SCREEN"] = knob
+    for (kn, knob), nm in zip(settings, names):
+        apply(kn, knob)
         for s in range(3):
             step(s)
         torch.cuda.synchronize()
@@ -89,25 +104,29 @@ for r in range(rounds):
         for s in range(steps):
             step(s)
         torch.cuda.synchronize()
-        res[knob].append(steps * B / (time.perf_counter() - t0))
+        res[nm].append(steps * B / (time.perf_counter() - t0))
         km = 0.0
         for s in range(4):
             step(s)
             km += idx.last_stats()["kernel_ms"]
-        kern[knob].append(km / 4)
-        print("round %d screen=%s  %.0f queries/s  kernel %.2f ms/step" % (r, knob, res[knob][-1], kern[knob][-1]), flush=True)
+        kern_ms[nm].append(km / 4)
+        print("round %d %s  %.0f queries/s  kernel %.2f ms/step" % (r, nm, res[nm][-1], kern_ms[nm][-1]), flush=True)
+auto = name("0", "auto")
 out = {"workload": wl_name, "data": data, "identical_outputs_and_counters": bool(same), "memory": mem,
-       "gpu": torch.cuda.get_device_name(0), "auto_screen_kind": ref["auto"][0][7], "auto_screen_dims": ref["auto"][0][8]}
-for knob in knobs:
-    v = np.array(res[knob])
-    cd = sum(o[3] for o in ref[knob])
-    fr = sum(o[6] for o in ref[knob])
-    out["screen_" + knob] = {"qps_median": float(np.median(v)), "qps_min": float(v.min()), "qps_max": float(v.max()),
-                             "kernel_ms_median": float(np.median(kern[knob])), "dist_evals_per_query": cd / (pool * B),
-                             "full_rows_read_per_query": fr / (pool * B), "full_rows_frac": fr / cd,
-                             "screen_kind": ref[knob][0][7], "codes_per_candidate": ref[knob][0][8]}
-for knob in knobs[1:]:
-    out["speedup_median_%s_vs_%s" % (knob, knobs[0])] = out["screen_" + knob]["qps_median"] / out["screen_" + knobs[0]]["qps_median"]
+       "gpu": torch.cuda.get_device_name(0), "auto_screen_kind": ref[auto][0][7], "auto_screen_dims": ref[auto][0][8],
+       "auto_search_kernel": ref[auto][0][9]}
+for nm in names:
+    v = np.array(res[nm])
+    cd = sum(o[3] for o in ref[nm])
+    fr = sum(o[6] for o in ref[nm])
+    cy = cyc[nm]
+    out[nm] = {"qps_median": float(np.median(v)), "qps_min": float(v.min()), "qps_max": float(v.max()),
+               "kernel_ms_median": float(np.median(kern_ms[nm])), "dist_evals_per_query": cd / (pool * B),
+               "full_rows_read_per_query": fr / (pool * B), "full_rows_frac": fr / cd,
+               "screen_kind": ref[nm][0][7], "codes_per_candidate": ref[nm][0][8], "search_kernel": ref[nm][0][9],
+               "cycle_split": {c[len("owner_cycles_"):]: (float(x / cy.sum()) if cy.sum() else 0.0) for c, x in zip(CYCLES, cy)}}
+for nm in names[1:]:
+    out["speedup_median_%s_vs_%s" % (nm, names[0])] = out[nm]["qps_median"] / out[names[0]]["qps_median"]
 print(json.dumps(out))
 if os.environ.get("OUT"):  # directory for the JSON result
     os.makedirs(os.environ["OUT"], exist_ok=True)

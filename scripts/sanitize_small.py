@@ -62,4 +62,19 @@ k3, d3, _ = grp.search_batch(Q, k)
 assert np.array_equal(k1, k3) and np.array_equal(d1.view(np.uint32), d3.view(np.uint32))
 grp.close()
 g.close()
+# the warp-per-query kernel with the projected screen (records, the per-batch pre-pass, q~ in the warp's shared memory)
+Xw = (rng.standard_normal((n, 16)) @ rng.standard_normal((16, 320)) + 0.05 * rng.standard_normal((n, 320))).astype(np.float32)
+os.environ["LB200_SEARCH_SCREEN"] = "2"
+g = api.Index(320, "cos", "f32", M=8, efc=32, ef=24)
+g.reserve(n)
+g.add_batch(np.arange(1, n + 1, dtype=np.uint64), Xw)
+g.build()
+g.set_option("search_kernel", 1)
+k1, d1, _ = g.search_batch(Xw[:nq], k)
+g.set_option("search_kernel", 2)
+k2, d2, _ = g.search_batch(Xw[:nq], k)
+assert g.last_stats()["screen_kind"] == 2
+assert np.array_equal(k1, k2) and np.array_equal(d1.view(np.uint32), d2.view(np.uint32))
+os.environ.pop("LB200_SEARCH_SCREEN")
+g.close()
 print("sanitize_small: done, %d kernel launches" % api.kernel_launches())
