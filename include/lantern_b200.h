@@ -308,16 +308,21 @@ LB200_EXPORT void lb200_merge_shards_device(lb200_key_t const* d_keys, lb200_dis
                                             lb200_distance_t* d_out_dists, void* cuda_stream, lb200_error_t* error);
 
 /* ---- multi-GPU: one graph searched by G GPUs ("row-sharded group", csrc/group.cu) ------------------------------------
- * The corpus is sharded by contiguous row range (SURVEY.md 8e): GPU r holds the vectors of rows [n*r/G, n*(r+1)/G) only.
- * The graph itself (adjacency lists, 4 B per link) is replicated, each query is walked ONCE in the reference's order, and
- * every distance is evaluated on the GPU that holds the row, over NVLink peer memory -- total work equals the 1-GPU
- * search, and so do the results (id for id on the same graph).  Two ways to form a group:
+ * The corpus is sharded by contiguous row range (SURVEY.md 8e): GPU r holds the vectors of rows [bounds[r], bounds[r+1])
+ * only.  The ranges are balanced by level-0 in-degree (rows that appear in more lists are measured more often), not equal
+ * in length; lb200_group_rank_info reports them.  The graph itself (adjacency lists, 4 B per link) is replicated, each query
+ * is walked ONCE in the reference's order, and every distance is evaluated on the GPU that holds the row, over NVLink peer
+ * memory -- total work equals the 1-GPU search, and so do the results (id for id on the same graph).  Two ways to create a
+ * group:
  *   lb200_group_create        one process per GPU (torchrun / MPI style); `allgather` is the caller's bootstrap collective
  *                             (every rank passes `bytes_per_rank` bytes, everybody receives world * bytes_per_rank, rank
  *                             order); it is used at creation/distribution time only, never on the search path;
  *   lb200_group_create_local  one process driving n devices (what a Lantern indexing/search server would do).
- * lb200_group_distribute: the root rank passes a built (or loaded) index that lives on ITS device; every rank copies its
- * row range and the graph from it over NVLink.  The root index is not modified and may be freed afterwards.  Collective.
+ * and two ways to give it its graph (once per group):
+ *   lb200_group_distribute    the root rank passes a built (or loaded) index that lives on ITS device; every rank copies its
+ *                             row range and the graph from it over NVLink.  The index must fit on one GPU.
+ *   lb200_group_load[_buffer] every rank reads its row range and the graph straight from an index file; no GPU ever holds
+ *                             all rows, so the group can serve an index larger than one GPU.
  * lb200_group_search_batch*: collective; only the root's queries are read (other ranks may pass NULL); EVERY rank receives
  * the full result (the final all-gather is fused into the kernel's epilogue: owners store their top-k into every rank). */
 typedef void* lb200_group_t;
@@ -343,6 +348,29 @@ LB200_EXPORT void lb200_group_free(lb200_group_t, lb200_error_t* error);
 /* max_batch: largest nq of a search; max_results: largest nq * count (sizes the peer-mapped staging buffers). */
 LB200_EXPORT void lb200_group_distribute(lb200_group_t, lb200_index_t root_index, int root, size_t max_batch,
                                          size_t max_results, lb200_error_t* error);
+/* Collective.  Forms the group's distribution from a usearch/lantern index file instead of from an index: every rank keeps
+ * the rows of its range and a copy of the graph; no rank ever holds all rows.  `options` is checked against the file exactly
+ * as lb200_load checks an index's options (metric, scalar kind, dimensions, connectivity; same messages) and supplies
+ * expansion_search.  root / max_batch / max_results: as in lb200_group_distribute.  PQ indexes are refused, as distribute
+ * refuses them.  The whole file is validated before any rank allocates: after a refusal the group can still take a correct
+ * load.  Rows travel through a bounded pinned staging block, so no host copy of the file is made.  Multi-process groups:
+ * every rank passes the same bytes (or the same path) and keeps its own range; a rank holding a different file fails the
+ * call on every rank.  A group takes one load or one distribute, not both. */
+LB200_EXPORT void lb200_group_load_buffer(lb200_group_t, lb200_init_options_t const* options, void const* buffer,
+                                          size_t length, int root, size_t max_batch, size_t max_results, lb200_error_t* error);
+/* the same from a file, mapped read-only (mmap): a file larger than host memory needs no more than its page cache */
+LB200_EXPORT void lb200_group_load(lb200_group_t, lb200_init_options_t const* options, char const* path, int root,
+                                   size_t max_batch, size_t max_results, lb200_error_t* error);
+/* What a rank keeps on its device, for a group formed either way.  bytes_scratch grows with max_batch * n: one visited
+ * bitmap of n bits per owner slot, and a rank has ceil(max_batch / world) slots (at most the resident warps). */
+typedef struct lb200_group_rank_info_t {
+    int rank, world;
+    uint64_t rows_begin, rows_end;         /* this rank's row range */
+    uint64_t bytes_rows, bytes_graph;      /* device bytes: its rows; adj0 + upper lists + keys */
+    uint64_t bytes_scratch, bytes_mailbox; /* visited bitmaps + touched lists + counters + query staging; the peer-mapped slab */
+} lb200_group_rank_info_t;
+/* local_rank: as in lb200_group_last_stats.  No device work. */
+LB200_EXPORT void lb200_group_rank_info(lb200_group_t, int local_rank, lb200_group_rank_info_t* info, lb200_error_t* error);
 /* lb200_group_build: inserts every pending (and staged) vector of `root_index`, which lives on the device of rank `root`,
  * with all ranks of a single-process group.  Every other rank works on a temporary replica of the index (freed when the call
  * returns); each batch's new nodes are split between the ranks, and every list is written into every replica over NVLink.

@@ -74,6 +74,12 @@ class GroupStats(C.Structure):
                 ("owner_cycles_wait", C.c_uint64), ("owner_cycles_consume", C.c_uint64)]
 
 
+class GroupRankInfo(C.Structure):
+    _fields_ = [("rank", C.c_int), ("world", C.c_int), ("rows_begin", C.c_uint64), ("rows_end", C.c_uint64),
+                ("bytes_rows", C.c_uint64), ("bytes_graph", C.c_uint64), ("bytes_scratch", C.c_uint64),
+                ("bytes_mailbox", C.c_uint64)]
+
+
 ALLGATHER_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t)
 ERRP = C.POINTER(C.c_char_p)
 
@@ -151,6 +157,10 @@ SIGNATURES = {
     "lb200_group_create_local": (C.c_void_p, [C.c_void_p, C.c_int, ERRP]),
     "lb200_group_free": (None, [C.c_void_p, ERRP]),
     "lb200_group_distribute": (None, [C.c_void_p, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, ERRP]),
+    "lb200_group_load_buffer": (None, [C.c_void_p, C.POINTER(InitOptions), C.c_void_p, C.c_size_t, C.c_int, C.c_size_t,
+                                       C.c_size_t, ERRP]),
+    "lb200_group_load": (None, [C.c_void_p, C.POINTER(InitOptions), C.c_char_p, C.c_int, C.c_size_t, C.c_size_t, ERRP]),
+    "lb200_group_rank_info": (None, [C.c_void_p, C.c_int, C.POINTER(GroupRankInfo), ERRP]),
     "lb200_group_build": (None, [C.c_void_p, C.c_void_p, C.c_int, ERRP]),
     "lb200_group_search_batch": (None, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_size_t, C.c_size_t,
                                         C.c_void_p, C.c_void_p, C.c_void_p, ERRP]),
@@ -199,6 +209,14 @@ def _ptr(x):
     return C.c_void_p(x.ctypes.data)
 
 
+def init_options(dim, metric="l2sq", quant="f32", M=16, efc=128, ef=64, pq=False, num_centroids=0, num_subvectors=0):
+    o = InitOptions()
+    o.metric_kind, o.quantization, o.dimensions = METRIC[metric], SCALAR[quant], dim
+    o.connectivity, o.expansion_add, o.expansion_search = M, efc, ef
+    o.pq, o.num_centroids, o.num_subvectors = pq, num_centroids, num_subvectors
+    return o
+
+
 class Index:
     """One HNSW index resident in the HBM of the current CUDA device."""
 
@@ -207,10 +225,7 @@ class Index:
         L = lib()
         self.dim, self.metric, self.quant, self.M = dim, metric, quant, M
         self.num_subvectors = num_subvectors
-        o = InitOptions()
-        o.metric_kind, o.quantization, o.dimensions = METRIC[metric], SCALAR[quant], dim
-        o.connectivity, o.expansion_add, o.expansion_search = M, efc, ef
-        o.pq, o.num_centroids, o.num_subvectors = pq, num_centroids, num_subvectors
+        o = init_options(dim, metric, quant, M, efc, ef, pq, num_centroids, num_subvectors)
         cb = None
         if codebook is not None:
             cb = np.ascontiguousarray(codebook, dtype=np.float32)
@@ -339,6 +354,7 @@ class Group:
     Group.local(devices)            one process driving len(devices) devices
     Group.ranked(rank, world, ag)   one process per GPU; `ag(send: bytes) -> bytes` is the caller's all-gather
                                     (concatenation of every rank's `send`, rank order), used for bootstrap only
+    then once: distribute(index) (an index on the root's GPU) or load(path) / load_buffer(bytes) (each rank reads its rows)
     """
 
     def __init__(self, handle, world, keep=None):
@@ -396,6 +412,26 @@ class Group:
 
     def distribute(self, index, root=0, max_batch=8192, max_results=0):
         self._call("lb200_group_distribute", index.h if index is not None else None, root, max_batch, max_results)
+
+    def load_buffer(self, buf, dim, metric="l2sq", quant="f32", M=16, efc=128, ef=64, pq=False, root=0, max_batch=8192,
+                    max_results=0):
+        """The group's graph straight from index file bytes (every rank passes the same bytes); the index options are those
+        of Index(...) and are checked against the file as Index.load_buffer checks them."""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        o = init_options(dim, metric, quant, M, efc, ef, pq)
+        self._call("lb200_group_load_buffer", C.byref(o), _ptr(buf), len(buf), root, max_batch, max_results)
+
+    def load(self, path, dim, metric="l2sq", quant="f32", M=16, efc=128, ef=64, pq=False, root=0, max_batch=8192,
+             max_results=0):
+        """load_buffer from a file, mapped read-only by the engine."""
+        o = init_options(dim, metric, quant, M, efc, ef, pq)
+        self._call("lb200_group_load", C.byref(o), path.encode(), root, max_batch, max_results)
+
+    def rank_info(self, local_rank=0):
+        """Row range and device bytes (rows, graph, scratch, mailbox) of a local rank."""
+        s = GroupRankInfo()
+        self._call("lb200_group_rank_info", local_rank, C.byref(s))
+        return {f: getattr(s, f) for f, _ in GroupRankInfo._fields_}
 
     def build(self, index, root=0):
         """Insert every pending vector of `index` (on rank `root`'s device) with all ranks: lb200_build's graph, byte for byte."""

@@ -4,8 +4,12 @@
 // error convention (static strings through `lb200_error_t*`, 0/NULL return on failure, no exception
 // crosses the ABI).  Every entry point is additionally exported under its reference name
 // (`usearch_*`) at the end of the file.
+#include <fcntl.h>
 #include <stdio.h>
 #include <string.h>
+#include <sys/mman.h>
+#include <sys/stat.h>
+#include <unistd.h>
 
 #include <algorithm>
 #include <mutex>
@@ -73,6 +77,53 @@ void check_metric_scalar(int metric, int scalar) {
         throw CudaError("hamming metric requires b1 scalars (dimensions in bits)");
 }
 
+// lb200_init's reading and checking of the options (a group load checks a file against them the same way)
+IndexConfig index_config(const lb200_init_options_t* options, const float* codebook) {
+    if (!options)
+        throw CudaError("null options");
+    require_device();
+    if (options->metric)
+        throw CudaError("custom metric callbacks cannot run on the GPU");
+    // options->retriever / retriever_mut / retriever_ctx: Lantern's build.c:512-517 always fills them before usearch_init
+    // ("retrievers are not called from here"); they only matter to usearch_view_mem_lazy / usearch_add_external, which
+    // refuse on their own.  Accepted and ignored here so that build.c runs unchanged.
+    if (options->multi)
+        throw CudaError("multi-vector keys are not supported");
+    if (options->pq) { // U/c/lib.cpp:135-140, lantern_storage.hpp:90-94
+        if (options->num_centroids == 0 || options->num_subvectors == 0)
+            throw CudaError("Must provide nonzero values for centroids and subvectors when pq-quantization option is set");
+        if (!codebook)
+            throw CudaError("pq index needs a codebook");
+        if (options->num_centroids > 256)
+            throw CudaError("number of centroids must fit in a byte");
+        if (options->dimensions % options->num_subvectors != 0)
+            throw CudaError("currently vector dimensions must be divisible to num_subvectors");
+        if (options->dimensions >= 2000)
+            throw CudaError("vectors larger than 2k dimensions not supported");
+        if (options->quantization != lb200_scalar_f32_k)
+            throw CudaError("pq index stores f32 codebooks only");
+    }
+    check_metric_scalar(options->metric_kind, options->quantization);
+    if (options->dimensions == 0)
+        throw CudaError("dimensions must be nonzero");
+    IndexConfig cfg;
+    cfg.metric_kind = options->metric_kind;
+    cfg.scalar_kind = options->quantization;
+    cfg.dims = options->dimensions;
+    cfg.M = options->connectivity ? options->connectivity : 16; // index.hpp:1249-1250
+    cfg.M0 = cfg.M * 2;
+    cfg.efc = options->expansion_add ? options->expansion_add : 128;
+    cfg.ef = options->expansion_search ? options->expansion_search : 64;
+    cfg.pq = options->pq;
+    cfg.num_centroids = options->num_centroids;
+    cfg.num_subvectors = options->num_subvectors;
+    if (cfg.M < 2 || cfg.M > 128)
+        throw CudaError("connectivity must be in [2, 128]"); // lantern_hnsw/src/hnsw/options.h:15-27
+    if (scalar_row_bytes(cfg.scalar_kind, cfg.dims) > 8192)
+        throw CudaError("vectors wider than 8192 bytes are not supported");
+    return cfg;
+}
+
 } // namespace
 
 extern "C" {
@@ -80,48 +131,7 @@ extern "C" {
 LB200_EXPORT lb200_index_t lb200_init(lb200_init_options_t* options, float* codebook, lb200_error_t* error) {
     lb200_index_t result = nullptr;
     guarded(error, [&] {
-        if (!options)
-            throw CudaError("null options");
-        require_device();
-        if (options->metric)
-            throw CudaError("custom metric callbacks cannot run on the GPU");
-        // options->retriever / retriever_mut / retriever_ctx: Lantern's build.c:512-517 always fills them before usearch_init
-        // ("retrievers are not called from here"); they only matter to usearch_view_mem_lazy / usearch_add_external, which
-        // refuse on their own.  Accepted and ignored here so that build.c runs unchanged.
-        if (options->multi)
-            throw CudaError("multi-vector keys are not supported");
-        if (options->pq) { // U/c/lib.cpp:135-140, lantern_storage.hpp:90-94
-            if (options->num_centroids == 0 || options->num_subvectors == 0)
-                throw CudaError("Must provide nonzero values for centroids and subvectors when pq-quantization option is set");
-            if (!codebook)
-                throw CudaError("pq index needs a codebook");
-            if (options->num_centroids > 256)
-                throw CudaError("number of centroids must fit in a byte");
-            if (options->dimensions % options->num_subvectors != 0)
-                throw CudaError("currently vector dimensions must be divisible to num_subvectors");
-            if (options->dimensions >= 2000)
-                throw CudaError("vectors larger than 2k dimensions not supported");
-            if (options->quantization != lb200_scalar_f32_k)
-                throw CudaError("pq index stores f32 codebooks only");
-        }
-        check_metric_scalar(options->metric_kind, options->quantization);
-        if (options->dimensions == 0)
-            throw CudaError("dimensions must be nonzero");
-        IndexConfig cfg;
-        cfg.metric_kind = options->metric_kind;
-        cfg.scalar_kind = options->quantization;
-        cfg.dims = options->dimensions;
-        cfg.M = options->connectivity ? options->connectivity : 16; // index.hpp:1249-1250
-        cfg.M0 = cfg.M * 2;
-        cfg.efc = options->expansion_add ? options->expansion_add : 128;
-        cfg.ef = options->expansion_search ? options->expansion_search : 64;
-        cfg.pq = options->pq;
-        cfg.num_centroids = options->num_centroids;
-        cfg.num_subvectors = options->num_subvectors;
-        if (cfg.M < 2 || cfg.M > 128)
-            throw CudaError("connectivity must be in [2, 128]"); // lantern_hnsw/src/hnsw/options.h:15-27
-        if (scalar_row_bytes(cfg.scalar_kind, cfg.dims) > 8192)
-            throw CudaError("vectors wider than 8192 bytes are not supported");
+        const IndexConfig cfg = index_config(options, codebook);
         result = new Index(cfg, codebook);
     });
     return result;
@@ -821,11 +831,80 @@ LB200_EXPORT lb200_group_t lb200_group_create_local(int const* devices, int n_de
 LB200_EXPORT void lb200_group_free(lb200_group_t h, lb200_error_t* error) {
     guarded(error, [&] { group_free(reinterpret_cast<Group*>(h)); });
 }
+static size_t group_max_batch(size_t max_batch) { return max_batch ? max_batch : 8192; }
+static size_t group_max_results(size_t max_batch, size_t max_results) {
+    return max_results ? max_results : group_max_batch(max_batch) * 128;
+}
 LB200_EXPORT void lb200_group_distribute(lb200_group_t h, lb200_index_t root_index, int root, size_t max_batch, size_t max_results,
                                          lb200_error_t* error) {
     guarded(error, [&] {
-        group_distribute(*as_group(h), reinterpret_cast<Index*>(root_index), root, max_batch ? max_batch : 8192,
-                         max_results ? max_results : (max_batch ? max_batch : 8192) * 128);
+        group_distribute(*as_group(h), reinterpret_cast<Index*>(root_index), root, group_max_batch(max_batch),
+                         group_max_results(max_batch, max_results));
+    });
+}
+// lb200_init's reading of the options; a group cannot hold PQ codes (distribute refuses PQ indexes the same way)
+static IndexConfig group_load_config(const lb200_init_options_t* options) {
+    if (options && options->pq)
+        throw CudaError("group: pq indexes are not supported");
+    return index_config(options, nullptr);
+}
+LB200_EXPORT void lb200_group_load_buffer(lb200_group_t h, lb200_init_options_t const* options, void const* buffer, size_t length,
+                                          int root, size_t max_batch, size_t max_results, lb200_error_t* error) {
+    guarded(error, [&] {
+        Group& G = *as_group(h);
+        const IndexConfig cfg = group_load_config(options);
+        if (!buffer && length)
+            throw CudaError("null buffer");
+        group_load(G, cfg, buffer, length, root, group_max_batch(max_batch), group_max_results(max_batch, max_results));
+    });
+}
+// A read-only mapping of a whole file: the pages are read as the load touches them, and may be dropped again by the kernel
+struct MappedFile {
+    int fd = -1;
+    void* p = MAP_FAILED;
+    size_t length = 0;
+    explicit MappedFile(const char* path) {
+        fd = open(path, O_RDONLY | O_CLOEXEC);
+        if (fd < 0)
+            throw CudaError("Can't open file for reading");
+        struct stat st;
+        if (fstat(fd, &st) != 0) {
+            close(fd);
+            throw CudaError("Failed to read the index file");
+        }
+        length = (size_t)st.st_size;
+        if (length) {
+            p = mmap(nullptr, length, PROT_READ, MAP_PRIVATE, fd, 0);
+            if (p == MAP_FAILED) {
+                close(fd);
+                throw CudaError("Failed to map the index file");
+            }
+            madvise(p, length, MADV_SEQUENTIAL);
+        }
+    }
+    ~MappedFile() {
+        if (p != MAP_FAILED)
+            munmap(p, length);
+        close(fd);
+    }
+    const void* data() const { return p == MAP_FAILED ? nullptr : p; }
+};
+LB200_EXPORT void lb200_group_load(lb200_group_t h, lb200_init_options_t const* options, char const* path, int root,
+                                   size_t max_batch, size_t max_results, lb200_error_t* error) {
+    guarded(error, [&] {
+        Group& G = *as_group(h);
+        const IndexConfig cfg = group_load_config(options);
+        if (!path)
+            throw CudaError("null path");
+        MappedFile f(path);
+        group_load(G, cfg, f.data(), f.length, root, group_max_batch(max_batch), group_max_results(max_batch, max_results));
+    });
+}
+LB200_EXPORT void lb200_group_rank_info(lb200_group_t h, int local_rank, lb200_group_rank_info_t* info, lb200_error_t* error) {
+    guarded(error, [&] {
+        if (!info)
+            throw CudaError("null info pointer");
+        group_rank_info(*as_group(h), local_rank, *info);
     });
 }
 LB200_EXPORT void lb200_group_build(lb200_group_t h, lb200_index_t root_index, int root, lb200_error_t* error) {

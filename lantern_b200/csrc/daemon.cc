@@ -2,7 +2,8 @@
 //
 // Why: a Postgres backend runs one query at a time (lantern_hnsw/src/hnsw/scan.c:64 num_threads = 1, :220-228 one
 // usearch_search_ef per scan) while the engine needs batches of ~1000 queries to reach the HBM roofline.  The daemon owns
-// one index handle (loaded from a usearch/lantern index file), accepts connections on a Unix-domain or TCP socket, collects
+// one index handle (loaded from a usearch/lantern index file; with --devices, a row-sharded group of GPUs loaded from it
+// instead), accepts connections on a Unix-domain or TCP socket, collects
 // the requests that arrive within a short window and serves them with ONE lb200_search_batch call per (k, ef) group.
 // It implements ldb_amgettuple's call pattern (scan.c:167-338): first fetch with k = init_k, then `continue` requests that
 // return the NEXT k results of the same query (never a row twice), per connection.
@@ -309,21 +310,25 @@ int main(int argc, char** argv) {
     o.quantization = (lb200_scalar_kind_t)parse_quant(quant);
     o.dimensions = dims, o.connectivity = m, o.expansion_add = efc, o.expansion_search = ef;
     lb200_error_t err = nullptr;
-    d.idx = lb200_init(&o, nullptr, &err);
-    if (err) {
-        fprintf(stderr, "lb200_init: %s\n", err);
-        return 1;
-    }
-    lb200_load(d.idx, index_path.c_str(), &err);
-    if (err) {
-        fprintf(stderr, "lb200_load: %s\n", err);
-        return 1;
-    }
     d.in_kind = o.quantization == lb200_scalar_b1_k ? lb200_scalar_b1_k : lb200_scalar_f32_k;
     d.qbytes = d.in_kind == lb200_scalar_b1_k ? (dims + 7) / 8 : dims * 4;
-    if (!devices.empty()) {
+    size_t vectors = 0;
+    if (devices.empty()) {
+        d.idx = lb200_init(&o, nullptr, &err);
+        if (err) {
+            fprintf(stderr, "lb200_init: %s\n", err);
+            return 1;
+        }
+        lb200_load(d.idx, index_path.c_str(), &err);
+        if (err) {
+            fprintf(stderr, "lb200_load: %s\n", err);
+            return 1;
+        }
+        vectors = lb200_size(d.idx, &err);
+    } else {
         // one graph over several GPUs: rows sharded by range, distances evaluated on the owning GPU, results identical to the
-        // single-GPU search (csrc/group.cu).  The loaded index is only the source of the distribution.
+        // single-GPU search (csrc/group.cu).  Every GPU reads its rows and the graph straight from the file: no GPU holds
+        // the whole index, so the file may be larger than one GPU.
         std::vector<int> devs;
         for (size_t at = 0; at < devices.size();) {
             devs.push_back(atoi(devices.c_str() + at));
@@ -334,12 +339,26 @@ int main(int argc, char** argv) {
         }
         d.group = lb200_group_create_local(devs.data(), (int)devs.size(), &err);
         if (!err) // streaming scans ask for up to 1000 rows per query (scan.c:249-252)
-            lb200_group_distribute(d.group, d.idx, 0, d.max_batch, d.max_batch * 1000, &err);
+            lb200_group_load(d.group, &o, index_path.c_str(), 0, d.max_batch, d.max_batch * 1000, &err);
         if (err) {
             fprintf(stderr, "lb200_group: %s\n", err);
             return 1;
         }
         fprintf(stderr, "lb200_search_daemon: serving from %zu GPUs (row-sharded group)\n", devs.size());
+        for (size_t r = 0; r < devs.size(); ++r) {
+            lb200_group_rank_info_t info;
+            lb200_group_rank_info(d.group, (int)r, &info, &err);
+            if (err) {
+                fprintf(stderr, "lb200_group_rank_info: %s\n", err);
+                return 1;
+            }
+            vectors = std::max<size_t>(vectors, info.rows_end);
+            fprintf(stderr,
+                    "lb200_search_daemon: rank %d on GPU %d: rows [%llu, %llu), device MB: rows %.1f, graph %.1f, scratch %.1f, "
+                    "mailbox %.1f\n",
+                    info.rank, devs[r], (unsigned long long)info.rows_begin, (unsigned long long)info.rows_end,
+                    info.bytes_rows / 1e6, info.bytes_graph / 1e6, info.bytes_scratch / 1e6, info.bytes_mailbox / 1e6);
+        }
     }
 
     int ls;
@@ -367,8 +386,8 @@ int main(int argc, char** argv) {
             return 1;
         }
     }
-    fprintf(stderr, "lb200_search_daemon: %zu vectors, batching up to %zu queries per %d us window\n", lb200_size(d.idx, &err),
-            d.max_batch, d.window_us);
+    fprintf(stderr, "lb200_search_daemon: %zu vectors, batching up to %zu queries per %d us window\n", vectors, d.max_batch,
+            d.window_us);
     std::thread batcher([&] { d.batcher(); });
     for (;;) {
         int fd = accept(ls, nullptr, nullptr);

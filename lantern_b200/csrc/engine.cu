@@ -64,9 +64,9 @@ template <typename T> void grow_device(T*& ptr, size_t old_count, size_t new_cou
 Index::Index(const IndexConfig& cfg, const float* codebook) : cfg_(cfg) {
     dist_mode_ = distance_mode(cfg.metric_kind, cfg.scalar_kind);
     vec_bytes_ = scalar_row_bytes(cfg.scalar_kind, cfg.dims);
+    row_bytes_ = stored_row_bytes(cfg);
     if (cfg.pq) {
         stored_bytes_ = cfg.num_subvectors;
-        row_bytes_ = round_up(cfg.num_subvectors, 16);
         LB_CUDA(cudaMalloc(&d_codebook_, cfg.num_centroids * cfg.dims * sizeof(float)));
         LB_CUDA(cudaMemcpy(d_codebook_, codebook, cfg.num_centroids * cfg.dims * sizeof(float), cudaMemcpyHostToDevice));
         LB_CUDA(cudaMalloc(&d_pq_pair_, cfg.num_subvectors * cfg.num_centroids * cfg.num_centroids * sizeof(float)));
@@ -76,7 +76,6 @@ Index::Index(const IndexConfig& cfg, const float* codebook) : cfg_(cfg) {
             throw CudaError("pq: num_subvectors * num_centroids look-up table does not fit in shared memory");
     } else {
         stored_bytes_ = vec_bytes_;
-        row_bytes_ = round_up(vec_bytes_, 16);
         if (cfg.scalar_kind == SK_F32 && (dist_mode_ == DM_L2SQ || dist_mode_ == DM_COS))
             sq_bytes_ = screen_code_bytes((uint32_t)row_bytes_);
         sq_on_ = sq_bytes_ != 0;
@@ -303,12 +302,17 @@ GraphView Index::view() const {
     g.sq_meta = d_sq_meta_;
     g.ps_records = reinterpret_cast<const uint4*>(d_ps_records_);
     g.ps_k = ps_k_;
+    g.flags = search_view_flags();
+    return g;
+}
+
+uint32_t search_view_flags() {
     // L2-prefetch the adjacency line of nodes that enter the top list (2); screened search rounds take both halves of a
     // 64-wide list in one bitmap-atomic round trip (8)
-    g.flags = 2u | 8u;
+    uint32_t flags = 2u | 8u;
     if (const char* e = getenv("LB200_FLAGS"))
-        g.flags = (uint32_t)atoi(e);
-    return g;
+        flags = (uint32_t)atoi(e);
+    return flags;
 }
 
 // Sized for the walks that stage the value in the CTA and build its table there -- every build kernel, and the search of a

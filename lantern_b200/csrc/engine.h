@@ -101,6 +101,29 @@ inline uint32_t pq_lut_width(size_t num_centroids, uint32_t max_code) {
     return (uint32_t)((num_centroids > 128 && max_code < 128) ? 128 : num_centroids);
 }
 
+// Bytes of one stored row in HBM: the vector (or PQ code) padded to whole 16-byte chunks
+inline size_t stored_row_bytes(const IndexConfig& cfg) {
+    return round_up(cfg.pq ? cfg.num_subvectors : scalar_row_bytes(cfg.scalar_kind, cfg.dims), 16);
+}
+// GraphView::flags of every search (LB200_FLAGS overrides the default; engine.cu)
+uint32_t search_view_flags();
+
+// A usearch/lantern index file, parsed and validated on the host against an index configuration (format.cu): the one parser
+// behind Index::load_buffer and the group's load.  Every check of the file happens here; the rows stay in the caller's buffer
+// (node i's stored bytes start at row_off[i]).
+struct ParsedIndexFile {
+    size_t n = 0;
+    uint32_t entry = 0;
+    int32_t max_level = -1;
+    std::vector<uint32_t> adj0, upper_ref, upper_adj; // the HBM layout (engine.h top): u32 ids, 0xFFFFFFFF padded
+    std::vector<int16_t> levels;
+    std::vector<uint64_t> keys;
+    std::vector<uint64_t> row_off;
+};
+// vec_bytes / stored_bytes: those of an index with `cfg` (Index::vec_bytes_, stored_bytes_)
+void parse_index_file(const IndexConfig& cfg, size_t vec_bytes, size_t stored_bytes, const void* buffer, size_t length,
+                      ParsedIndexFile& out);
+
 struct SearchScratch {
     uint32_t* visited;     // [ctas][words_per_cta]
     uint32_t* touched;     // [ctas][touched_cap]

@@ -149,38 +149,33 @@ size_t Index::save_buffer(void* buffer, size_t length) {
     return (size_t)(p - (uint8_t*)buffer);
 }
 
-// usearch_load_buffer / usearch_view_buffer (U/c/lib.cpp:295-313): replaces the index contents.
-void Index::load_buffer(const void* buffer, size_t length) {
-    {
-        std::lock_guard<std::mutex> sg(stage_mu_); // loading replaces the contents, staged rows included
-        staged_rows_.clear(), staged_keys_.clear();
-    }
-    std::lock_guard<std::mutex> g(mu_);
+void parse_index_file(const IndexConfig& cfg, size_t vec_bytes, size_t stored_bytes, const void* buffer, size_t length,
+                      ParsedIndexFile& out) {
     const uint8_t* p = (const uint8_t*)buffer;
     if (length < 136 || memcmp(p, "usearch", 7) != 0)
         throw CudaError("index file: bad magic");
     if (p[15] != 8 || p[16] != 16)
         throw CudaError("index file: expected u64 keys and uint48 slots (lantern storage)");
-    if (p[13] != metric_char(cfg_.metric_kind) || p[14] != scalar_code(cfg_.scalar_kind))
+    if (p[13] != metric_char(cfg.metric_kind) || p[14] != scalar_code(cfg.scalar_kind))
         throw CudaError("index file: metric / scalar kind differ from the index options");
     uint64_t dims;
     memcpy(&dims, p + 33, 8);
-    if (dims != cfg_.dims)
+    if (dims != cfg.dims)
         throw CudaError("index file: dimensions differ from the index options");
     uint64_t hdr[7];
     memcpy(hdr, p + 80, 56);
-    const size_t n = hdr[0], M = cfg_.M, M0 = cfg_.M0;
+    const size_t n = hdr[0], M = cfg.M, M0 = cfg.M0;
     if (hdr[1] != M || hdr[2] != M0)
         throw CudaError("index file: connectivity differs from the index options");
-    if (hdr[5] != vec_bytes_)
+    if (hdr[5] != vec_bytes)
         throw CudaError("index file: vector_size_bytes mismatch");
     if (n >= 0x7FFFFFFFull)
         throw CudaError("index file: more than 2^31-1 nodes in one shard");
 
     std::vector<uint32_t> adj0(n * M0), upper_ref(n, kNoNeighbor), upper_adj;
-    std::vector<uint8_t> rows(n * row_bytes_, 0);
     std::vector<int16_t> levels(n);
-    std::vector<uint64_t> keys(n);
+    std::vector<uint64_t> keys(n), row_off(n);
+    const uint8_t* begin = p;
     const uint8_t* end = p + length;
     p += 136;
     std::vector<uint32_t> tmp(M);
@@ -192,7 +187,7 @@ void Index::load_buffer(const void* buffer, size_t length) {
         p += 10;
         if (levels[i] < 0)
             throw CudaError("index file: negative level");
-        const size_t tape = (4 + 6 * M0) + (size_t)levels[i] * (4 + 6 * M) + stored_bytes_;
+        const size_t tape = (4 + 6 * M0) + (size_t)levels[i] * (4 + 6 * M) + stored_bytes;
         if (p + tape > end)
             throw CudaError("index file: truncated");
         p = get_list(p, adj0.data() + i * M0, M0, n);
@@ -203,8 +198,8 @@ void Index::load_buffer(const void* buffer, size_t length) {
                 upper_adj.insert(upper_adj.end(), tmp.begin(), tmp.end());
             }
         }
-        memcpy(rows.data() + i * row_bytes_, p, stored_bytes_);
-        p += stored_bytes_;
+        row_off[i] = (uint64_t)(p - begin);
+        p += stored_bytes;
     }
     if (n) { // the walk starts at entry_slot on level max_level: both must be consistent or the kernels would read out of bounds
         if (hdr[4] >= n)
@@ -222,6 +217,30 @@ void Index::load_buffer(const void* buffer, size_t length) {
             }
         }
     }
+    out.n = n;
+    out.max_level = n ? (int32_t)hdr[3] : -1;
+    out.entry = (uint32_t)hdr[4];
+    out.adj0 = std::move(adj0), out.upper_ref = std::move(upper_ref), out.upper_adj = std::move(upper_adj);
+    out.levels = std::move(levels), out.keys = std::move(keys), out.row_off = std::move(row_off);
+}
+
+// usearch_load_buffer / usearch_view_buffer (U/c/lib.cpp:295-313): replaces the index contents.
+void Index::load_buffer(const void* buffer, size_t length) {
+    {
+        std::lock_guard<std::mutex> sg(stage_mu_); // loading replaces the contents, staged rows included
+        staged_rows_.clear(), staged_keys_.clear();
+    }
+    std::lock_guard<std::mutex> g(mu_);
+    ParsedIndexFile f;
+    parse_index_file(cfg_, vec_bytes_, stored_bytes_, buffer, length, f);
+    const size_t n = f.n, M = cfg_.M, M0 = cfg_.M0;
+    const std::vector<uint32_t>& adj0 = f.adj0;
+    const std::vector<uint32_t>& upper_ref = f.upper_ref;
+    const std::vector<uint32_t>& upper_adj = f.upper_adj;
+    std::vector<uint64_t>& keys = f.keys;
+    std::vector<uint8_t> rows(n * row_bytes_, 0);
+    for (size_t i = 0; i < n; ++i)
+        memcpy(rows.data() + i * row_bytes_, (const uint8_t*)buffer + f.row_off[i], stored_bytes_);
     uint32_t pq_max_code = 0;
     if (cfg_.pq) { // codes written by other tools may use all 256 centroids: size the look-up tables accordingly
         for (size_t i = 0; i < n; ++i)
@@ -255,11 +274,11 @@ void Index::load_buffer(const void* buffer, size_t length) {
         LB_CUDA(cudaMemcpy(d_keys_, keys.data(), keys.size() * 8, cudaMemcpyHostToDevice));
     }
     upper_lists_ = upper_adj.size() / M;
-    h_levels_ = std::move(levels);
+    h_levels_ = std::move(f.levels);
     h_keys_ = std::move(keys);
     n_ = n;
-    max_level_ = n ? (int32_t)hdr[3] : -1;
-    entry_ = (uint32_t)hdr[4];
+    max_level_ = f.max_level;
+    entry_ = f.entry;
     decide_screen();
 }
 

@@ -978,6 +978,90 @@ static SlabLayout slab_layout(uint32_t Omax, uint32_t G, uint32_t cap, size_t re
     return s;
 }
 
+// Contiguous row ranges (SURVEY 8e) of equal expected work, from the level-0 in-degree per bucket of kBalanceBuckets
+// consecutive rows (indegree_hist_kernel on an index, host_indegree_hist on a parsed file: the same counts).
+static void balanced_bounds(const std::vector<unsigned long long>& hist, size_t n_rows, int world, uint32_t* bounds) {
+    // weight of a bucket = its in-degree + the mean in-degree: measured on the bench corpus, equal-length ranges leave the
+    // first of two ranks 58 % of the evaluations, pure in-degree weighting 45 %; the blend lands near 50 %
+    double links = 0;
+    for (unsigned long long h : hist)
+        links += (double)h;
+    const double mean = links / kBalanceBuckets + 1.0;
+    double total = 0;
+    for (unsigned long long h : hist)
+        total += (double)h + mean;
+    bounds[0] = 0;
+    double acc = 0;
+    int r = 1;
+    for (uint32_t b = 0; b < kBalanceBuckets && r < world; ++b) {
+        acc += (double)hist[b] + mean;
+        while (r < world && acc >= total * r / world) {
+            bounds[r] = (uint32_t)std::min<size_t>(n_rows, ((size_t)(b + 1) * n_rows + kBalanceBuckets - 1) / kBalanceBuckets);
+            ++r;
+        }
+    }
+    for (; r <= world; ++r)
+        bounds[r] = (uint32_t)n_rows;
+    bounds[world] = (uint32_t)n_rows;
+    if (getenv("LB200_GROUP_EQUAL_RANGES")) // experiments: plain n*r/G ranges
+        for (int q = 0; q <= world; ++q)
+            bounds[q] = (uint32_t)((n_rows * (size_t)q) / (size_t)world);
+    for (int q = 1; q <= world; ++q) // monotone, whatever the histogram looked like
+        bounds[q] = std::max(bounds[q], bounds[q - 1]);
+}
+
+static std::vector<unsigned long long> host_indegree_hist(const std::vector<uint32_t>& adj0, size_t n) {
+    std::vector<unsigned long long> hist(kBalanceBuckets, 0);
+    for (uint32_t id : adj0)
+        if (id < n)
+            hist[(uint32_t)(((unsigned long long)id * kBalanceBuckets) / n)] += 1;
+    return hist;
+}
+
+// Rows [lo, hi) of a file (node i's stored bytes at file + row_off[i]) into d_rows on the current device, row_bytes apart and
+// zero padded.  Rows are gathered into one half of a bounded pinned block while the other half is on its way to the device:
+// no host copy of a whole slice (or file) is ever made.
+static void upload_file_rows(const uint8_t* file, const std::vector<uint64_t>& row_off, size_t stored_bytes, size_t lo, size_t hi,
+                             uint8_t* d_rows, size_t row_bytes) {
+    if (hi <= lo)
+        return;
+    struct Staging {
+        uint8_t* pinned = nullptr;
+        cudaStream_t stream = nullptr;
+        cudaEvent_t done[2] = {nullptr, nullptr};
+        ~Staging() {
+            if (stream)
+                cudaStreamSynchronize(stream), cudaStreamDestroy(stream);
+            for (cudaEvent_t e : done)
+                if (e)
+                    cudaEventDestroy(e);
+            if (pinned)
+                cudaFreeHost(pinned);
+        }
+    } st;
+    const size_t block = std::max<size_t>(1, std::min(hi - lo, ((size_t)32 << 20) / row_bytes)); // rows per half (<= 32 MB)
+    LB_CUDA(cudaMallocHost(&st.pinned, 2 * block * row_bytes));
+    LB_CUDA(cudaStreamCreateWithFlags(&st.stream, cudaStreamNonBlocking));
+    LB_CUDA(cudaEventCreateWithFlags(&st.done[0], cudaEventDisableTiming));
+    LB_CUDA(cudaEventCreateWithFlags(&st.done[1], cudaEventDisableTiming));
+    bool used[2] = {false, false};
+    int h = 0;
+    for (size_t b0 = lo; b0 < hi; b0 += block, h ^= 1) {
+        const size_t cnt = std::min(block, hi - b0);
+        uint8_t* stage = st.pinned + (size_t)h * block * row_bytes;
+        if (used[h])
+            LB_CUDA(cudaEventSynchronize(st.done[h]));
+        for (size_t i = 0; i < cnt; ++i) {
+            memcpy(stage + i * row_bytes, file + row_off[b0 + i], stored_bytes);
+            memset(stage + i * row_bytes + stored_bytes, 0, row_bytes - stored_bytes);
+        }
+        LB_CUDA(cudaMemcpyAsync(d_rows + (b0 - lo) * row_bytes, stage, cnt * row_bytes, cudaMemcpyHostToDevice, st.stream));
+        LB_CUDA(cudaEventRecord(st.done[h], st.stream));
+        used[h] = true;
+    }
+    LB_CUDA(cudaStreamSynchronize(st.stream));
+}
+
 class GroupRank {
   public:
     int rank = 0, world = 1, device = 0;
@@ -1017,12 +1101,32 @@ class GroupRank {
         cudaSetDevice(device);
         for (void* p : opened)
             cudaIpcCloseMemHandle(p);
+        release();
+    }
+
+    // what allocate() takes on this rank's device (lb200_group_rank_info_t)
+    void footprint(lb200_group_rank_info_t& f) const {
+        memset(&f, 0, sizeof(f));
+        f.rank = rank, f.world = world;
+        f.rows_begin = bounds[rank], f.rows_end = bounds[rank + 1];
+        f.bytes_rows = (f.rows_end - f.rows_begin) * row_bytes;
+        f.bytes_graph = n * cfg.M0 * 4 + n * 4 + upper_lists * cfg.M * 4 + n * 8;
+        f.bytes_scratch = (size_t)Omax * words_per_slot * 4 + (size_t)Omax * touched_cap * 4 + 16 * sizeof(unsigned long long) + in_bytes;
+        f.bytes_mailbox = lay.total;
+    }
+
+    // frees every device allocation of the rank (its peer mappings stay)
+    void release() {
+        cudaSetDevice(device);
         cudaFree(d_rows), cudaFree(d_adj0), cudaFree(d_upper_ref), cudaFree(d_upper_adj), cudaFree(d_keys);
         cudaFree(slab), cudaFree(d_vis), cudaFree(d_touched), cudaFree(d_counters), cudaFree(d_in);
+        d_rows = nullptr, d_adj0 = d_upper_ref = d_upper_adj = nullptr, d_keys = nullptr;
+        slab = nullptr, d_vis = d_touched = nullptr, d_counters = nullptr, d_in = nullptr;
         if (ev0)
             cudaEventDestroy(ev0);
         if (ev1)
             cudaEventDestroy(ev1);
+        ev0 = ev1 = nullptr;
     }
 
     PtrBlob export_ptr(void* p) const {
@@ -1081,34 +1185,7 @@ class GroupRank {
             std::vector<unsigned long long> hist(kBalanceBuckets);
             LB_CUDA(cudaMemcpy(hist.data(), d_hist, hist.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
             LB_CUDA(cudaFree(d_hist));
-            // weight of a bucket = its in-degree + the mean in-degree: measured on the bench corpus, equal-length ranges leave the
-            // first of two ranks 58 % of the evaluations, pure in-degree weighting 45 %; the blend lands near 50 %
-            double links = 0;
-            for (unsigned long long h : hist)
-                links += (double)h;
-            const double mean = links / kBalanceBuckets + 1.0;
-            double total = 0;
-            for (unsigned long long h : hist)
-                total += (double)h + mean;
-            const size_t n_rows = idx->n_;
-            c.bounds[0] = 0;
-            double acc = 0;
-            int r = 1;
-            for (uint32_t b = 0; b < kBalanceBuckets && r < world; ++b) {
-                acc += (double)hist[b] + mean;
-                while (r < world && acc >= total * r / world) {
-                    c.bounds[r] = (uint32_t)std::min<size_t>(n_rows, ((size_t)(b + 1) * n_rows + kBalanceBuckets - 1) / kBalanceBuckets);
-                    ++r;
-                }
-            }
-            for (; r <= world; ++r)
-                c.bounds[r] = (uint32_t)n_rows;
-            c.bounds[world] = (uint32_t)n_rows;
-            if (getenv("LB200_GROUP_EQUAL_RANGES")) // experiments: plain n*r/G ranges
-                for (int q = 0; q <= world; ++q)
-                    c.bounds[q] = (uint32_t)((n_rows * (size_t)q) / (size_t)world);
-            for (int q = 1; q <= world; ++q) // monotone, whatever the histogram looked like
-                c.bounds[q] = std::max(c.bounds[q], c.bounds[q - 1]);
+            balanced_bounds(hist, idx->n_, world, c.bounds);
         }
         c.vectors = export_ptr(idx->d_vectors_), c.adj0 = export_ptr(idx->d_adj0_);
         c.upper_ref = export_ptr(idx->d_upper_ref_), c.upper_adj = export_ptr(idx->d_upper_adj_);
@@ -1116,10 +1193,8 @@ class GroupRank {
         return c;
     }
 
-    PtrBlob adopt(const GroupConfigBlob& c, int root, size_t max_batch_, size_t max_results) {
-        if (!c.valid)
-            throw CudaError("group: the root rank passed no index");
-        LB_CUDA(cudaSetDevice(device));
+    // the graph's description, from the root's index (distribute) or from a file (load)
+    void configure(const GroupConfigBlob& c) {
         cfg = IndexConfig();
         cfg.metric_kind = c.metric_kind, cfg.scalar_kind = c.scalar_kind;
         cfg.dims = c.dims, cfg.M = c.M, cfg.M0 = c.M0, cfg.ef = c.ef;
@@ -1129,13 +1204,68 @@ class GroupRank {
         if (cfg.M0 > 256)
             throw CudaError("group: connectivity above 128 is not supported");
         for (int r = 0; r <= world; ++r)
-            bounds[r] = c.bounds[r]; // contiguous row ranges (SURVEY 8e), sized by the root for equal expected work
+            bounds[r] = c.bounds[r]; // contiguous row ranges (SURVEY 8e), sized for equal expected work
+    }
+
+    template <typename T> void device_alloc(T** p, size_t bytes, const char* what) {
+        const cudaError_t e = cudaMalloc((void**)p, bytes);
+        if (e == cudaSuccess)
+            return;
+        (void)cudaGetLastError();
+        size_t free_b = 0, total_b = 0;
+        if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess)
+            (void)cudaGetLastError();
+        throw CudaError("group: rank " + std::to_string(rank) + " (device " + std::to_string(device) + "): no room for its " + what +
+                        ": " + std::to_string(bytes) + " bytes requested, " + std::to_string(free_b) + " free (" + cudaGetErrorString(e) + ")");
+    }
+
+    // Everything the rank keeps on its device, taken at once: no cudaMalloc may happen between the launches of a search (it
+    // may wait for kernels already running on this device, and those kernels wait for the rank that is allocating).  On a
+    // failure nothing stays allocated and the error names what did not fit: rows, graph, mailbox or scratch
+    // (lb200_group_rank_info_t).
+    void allocate(size_t max_batch_, size_t max_results) {
+        LB_CUDA(cudaSetDevice(device));
+        int sms = 0;
+        LB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+        cap = (uint32_t)cfg.M0;
+        Wmax = (uint32_t)sms * 8u * kGroupWarps; // upper bound of resident warps (8 CTAs per SM)
+        max_batch = max_batch_, res_cap = max_results;
+        // owner slots: one per query a rank owns in the largest batch (never more than the resident warps)
+        Omax = (uint32_t)std::min<size_t>(Wmax, round_up((max_batch + world - 1) / world, kGroupWarps));
+        lay = slab_layout(Omax, (uint32_t)world, cap, res_cap, max_batch, row_bytes);
+        words_per_slot = round_up((n + 31) / 32, 32); // owner scratch: one visited bitmap per owned slot
+        // staging of raw input queries for the host-buffer entry point
+        in_bytes = max_batch * std::max<size_t>(row_bytes, cfg.dims * 4);
+        const size_t lo = bounds[rank], hi = bounds[rank + 1], owned = Omax;
+        try {
+            device_alloc(&d_rows, std::max<size_t>((hi - lo) * row_bytes, 16), "rows");
+            device_alloc(&d_adj0, n * cfg.M0 * 4, "graph (lists, keys)");
+            device_alloc(&d_upper_ref, n * 4, "graph (lists, keys)");
+            device_alloc(&d_upper_adj, std::max<size_t>(upper_lists * cfg.M * 4, 16), "graph (lists, keys)");
+            device_alloc(&d_keys, n * 8, "graph (lists, keys)");
+            device_alloc(&slab, lay.total, "mailbox");
+            device_alloc(&d_vis, owned * words_per_slot * 4, "scratch (visited bitmaps)");
+            device_alloc(&d_touched, owned * (size_t)touched_cap * 4, "scratch (touched lists)");
+            device_alloc(&d_counters, 16 * sizeof(unsigned long long), "scratch (counters)");
+            device_alloc(&d_in, in_bytes, "scratch (query staging)");
+            LB_CUDA(cudaMemset(slab, 0, lay.total));
+            LB_CUDA(cudaMemset(d_vis, 0, owned * words_per_slot * 4));
+            LB_CUDA(cudaMemset(d_counters, 0, 16 * sizeof(unsigned long long)));
+            LB_CUDA(cudaEventCreate(&ev0));
+            LB_CUDA(cudaEventCreate(&ev1));
+        } catch (...) {
+            release();
+            throw;
+        }
+    }
+
+    PtrBlob adopt(const GroupConfigBlob& c, int root, size_t max_batch_, size_t max_results) {
+        if (!c.valid)
+            throw CudaError("group: the root rank passed no index");
+        LB_CUDA(cudaSetDevice(device));
+        configure(c);
+        allocate(max_batch_, max_results);
         const size_t lo = bounds[rank], hi = bounds[rank + 1];
-        LB_CUDA(cudaMalloc(&d_rows, std::max<size_t>((hi - lo) * row_bytes, 16)));
-        LB_CUDA(cudaMalloc(&d_adj0, n * cfg.M0 * 4));
-        LB_CUDA(cudaMalloc(&d_upper_ref, n * 4));
-        LB_CUDA(cudaMalloc(&d_upper_adj, std::max<size_t>(upper_lists * cfg.M * 4, 16)));
-        LB_CUDA(cudaMalloc(&d_keys, n * 8));
         auto fetch = [&](void* dst, const PtrBlob& b, size_t offset, size_t bytes) {
             if (!bytes)
                 return;
@@ -1148,33 +1278,20 @@ class GroupRank {
         fetch(d_upper_ref, c.upper_ref, 0, n * 4);
         fetch(d_upper_adj, c.upper_adj, 0, upper_lists * cfg.M * 4);
         fetch(d_keys, c.keys, 0, n * 8);
-        // mailboxes
-        int sms = 0;
-        LB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-        cap = (uint32_t)cfg.M0;
-        Wmax = (uint32_t)sms * 8u * kGroupWarps; // upper bound of resident warps (8 CTAs per SM)
-        max_batch = max_batch_, res_cap = max_results;
-        // owner slots: one per query a rank owns in the largest batch (never more than the resident warps)
-        Omax = (uint32_t)std::min<size_t>(Wmax, round_up((max_batch + world - 1) / world, kGroupWarps));
-        lay = slab_layout(Omax, (uint32_t)world, cap, res_cap, max_batch, row_bytes);
-        LB_CUDA(cudaMalloc(&slab, lay.total));
-        LB_CUDA(cudaMemset(slab, 0, lay.total));
-        // owner scratch: one visited bitmap per owned slot
-        words_per_slot = round_up((n + 31) / 32, 32);
-        const size_t owned = Omax;
-        LB_CUDA(cudaMalloc(&d_vis, owned * words_per_slot * 4));
-        LB_CUDA(cudaMemset(d_vis, 0, owned * words_per_slot * 4));
-        LB_CUDA(cudaMalloc(&d_touched, owned * (size_t)touched_cap * 4));
-        LB_CUDA(cudaMalloc(&d_counters, 16 * sizeof(unsigned long long)));
-        LB_CUDA(cudaMemset(d_counters, 0, 16 * sizeof(unsigned long long)));
-        // staging of raw input queries for the host-buffer entry point: allocated NOW -- a cudaMalloc between the launches of a
-        // search may wait for kernels already running on this device, and those kernels wait for the rank that is allocating
-        in_bytes = max_batch * std::max<size_t>(row_bytes, cfg.dims * 4);
-        LB_CUDA(cudaMalloc(&d_in, in_bytes));
-        LB_CUDA(cudaEventCreate(&ev0));
-        LB_CUDA(cudaEventCreate(&ev1));
         LB_CUDA(cudaDeviceSynchronize());
         return export_ptr(slab);
+    }
+
+    // load: this rank's rows from the caller's file bytes, the graph from the parsed lists
+    void fill_from_file(const ParsedIndexFile& f, const uint8_t* file, size_t stored_bytes) {
+        LB_CUDA(cudaSetDevice(device));
+        upload_file_rows(file, f.row_off, stored_bytes, bounds[rank], bounds[rank + 1], d_rows, row_bytes);
+        LB_CUDA(cudaMemcpy(d_adj0, f.adj0.data(), f.adj0.size() * 4, cudaMemcpyHostToDevice));
+        LB_CUDA(cudaMemcpy(d_upper_ref, f.upper_ref.data(), f.upper_ref.size() * 4, cudaMemcpyHostToDevice));
+        if (!f.upper_adj.empty())
+            LB_CUDA(cudaMemcpy(d_upper_adj, f.upper_adj.data(), f.upper_adj.size() * 4, cudaMemcpyHostToDevice));
+        LB_CUDA(cudaMemcpy(d_keys, f.keys.data(), f.keys.size() * 8, cudaMemcpyHostToDevice));
+        LB_CUDA(cudaDeviceSynchronize());
     }
 
     void map_peers(const PtrBlob* slabs) {
@@ -1365,9 +1482,15 @@ void group_distribute(Group& G, Index* root_index, int root, size_t max_batch, s
     memcpy(&cfg, all.data() + (size_t)root * sizeof(GroupConfigBlob), sizeof(cfg));
     // B: every rank copies its row range and the graph from the root, allocates its mailboxes
     std::vector<std::vector<uint8_t>> slabs(nr, std::vector<uint8_t>(sizeof(PtrBlob)));
-    for (size_t i = 0; i < nr; ++i) {
-        PtrBlob b = G.ranks[i]->adopt(cfg, root, max_batch, max_results);
-        memcpy(slabs[i].data(), &b, sizeof(b));
+    try {
+        for (size_t i = 0; i < nr; ++i) {
+            PtrBlob b = G.ranks[i]->adopt(cfg, root, max_batch, max_results);
+            memcpy(slabs[i].data(), &b, sizeof(b));
+        }
+    } catch (...) {
+        for (GroupRank* r : G.ranks)
+            r->release();
+        throw;
     }
     G.exchange(slabs, all, sizeof(PtrBlob)); // also tells the root that everybody is done reading its index
     // C: map the peers' mailboxes
@@ -1377,6 +1500,136 @@ void group_distribute(Group& G, Index* root_index, int root, size_t max_batch, s
     G.exchange(tick, all, 4); // nobody searches before everybody has mapped everybody
     G.root = root;
     G.distributed = true;
+}
+
+// What every rank of a load reports before anything is allocated: whether its file parsed, and what it holds
+struct GroupFileBlob {
+    uint32_t ok;
+    uint8_t header[136];
+    uint64_t n, checksum;
+    char error[256];
+};
+// What every rank reports after allocating and filling its share: its mailbox slab, or why it could not
+struct GroupSlabBlob {
+    PtrBlob slab;
+    uint32_t ok;
+    char error[256];
+};
+
+// keys, levels and lists of a parsed file: two ranks that hold different files with equal headers still disagree here
+static uint64_t graph_checksum(const ParsedIndexFile& f) {
+    uint64_t h = 1469598103934665603ull;
+    auto mix = [&h](uint64_t v) { h = (h ^ v) * 1099511628211ull; };
+    for (size_t i = 0; i < f.n; ++i)
+        mix(f.keys[i]), mix((uint64_t)(uint16_t)f.levels[i]);
+    for (uint32_t v : f.adj0)
+        mix(v);
+    for (uint32_t v : f.upper_adj)
+        mix(v);
+    return h;
+}
+
+void group_load(Group& G, const IndexConfig& cfg, const void* buffer, size_t length, int root, size_t max_batch,
+                size_t max_results) {
+    DeviceGuard dg;
+    std::lock_guard<std::mutex> lk(G.mu);
+    if (G.distributed)
+        throw CudaError("group: already distributed");
+    if (root < 0 || root >= G.world)
+        throw CudaError("group: bad root rank");
+    const size_t nr = G.ranks.size();
+    const bool one_process = nr == (size_t)G.world;
+    const size_t vec_bytes = scalar_row_bytes(cfg.scalar_kind, cfg.dims);
+    // A: parse and check the file (once per process) before anything is allocated; then make sure every rank holds the same one
+    ParsedIndexFile f;
+    GroupFileBlob mine;
+    memset(&mine, 0, sizeof(mine));
+    try {
+        parse_index_file(cfg, vec_bytes, vec_bytes, buffer, length, f);
+        if (f.n == 0)
+            throw CudaError("group: the index is empty");
+        mine.ok = 1;
+        memcpy(mine.header, buffer, 136);
+        mine.n = f.n, mine.checksum = graph_checksum(f);
+    } catch (const std::exception& e) {
+        if (one_process)
+            throw; // (nobody else to tell)
+        snprintf(mine.error, sizeof(mine.error), "%s", e.what());
+    }
+    std::vector<std::vector<uint8_t>> blobs(nr, std::vector<uint8_t>(sizeof(GroupFileBlob)));
+    for (size_t i = 0; i < nr; ++i)
+        memcpy(blobs[i].data(), &mine, sizeof(mine));
+    std::vector<uint8_t> all;
+    G.exchange(blobs, all, sizeof(GroupFileBlob));
+    if (!mine.ok)
+        throw CudaError(mine.error);
+    for (int r = 0; r < G.world; ++r) {
+        GroupFileBlob o;
+        memcpy(&o, all.data() + (size_t)r * sizeof(GroupFileBlob), sizeof(o));
+        if (!o.ok)
+            throw CudaError("group: rank " + std::to_string(r) + " could not load its index file: " + o.error);
+        if (memcmp(o.header, mine.header, 136) != 0 || o.n != mine.n || o.checksum != mine.checksum)
+            throw CudaError("group: the ranks passed different index files (rank " + std::to_string(r) + " differs from rank " +
+                            std::to_string(G.ranks[0]->rank) + ")");
+    }
+    // the description an index with these options would give (GroupRank::describe)
+    GroupConfigBlob c;
+    memset(&c, 0, sizeof(c));
+    c.valid = 1;
+    c.metric_kind = cfg.metric_kind, c.scalar_kind = cfg.scalar_kind;
+    c.dims = cfg.dims, c.M = cfg.M, c.M0 = cfg.M0, c.ef = cfg.ef;
+    c.n = f.n, c.upper_lists = f.upper_adj.size() / cfg.M, c.row_bytes = stored_row_bytes(cfg), c.vec_bytes = vec_bytes;
+    c.entry = f.entry, c.max_level = f.max_level;
+    c.flags = search_view_flags();
+    balanced_bounds(host_indegree_hist(f.adj0, f.n), f.n, G.world, c.bounds);
+    // B: every rank allocates and fills its share; the mailbox exchange also carries whether that worked
+    std::vector<std::vector<uint8_t>> slabs(nr, std::vector<uint8_t>(sizeof(GroupSlabBlob), 0));
+    for (size_t i = 0; i < nr; ++i) {
+        GroupRank* r = G.ranks[i];
+        GroupSlabBlob b;
+        memset(&b, 0, sizeof(b));
+        try {
+            LB_CUDA(cudaSetDevice(r->device));
+            r->configure(c);
+            r->allocate(max_batch, max_results);
+            r->fill_from_file(f, (const uint8_t*)buffer, vec_bytes);
+            b.slab = r->export_ptr(r->slab);
+            b.ok = 1;
+        } catch (const std::exception& e) {
+            snprintf(b.error, sizeof(b.error), "%s", e.what());
+        }
+        memcpy(slabs[i].data(), &b, sizeof(b));
+        if (!b.ok)
+            break; // (the ranks after it report neither success nor a reason)
+    }
+    G.exchange(slabs, all, sizeof(GroupSlabBlob));
+    std::vector<PtrBlob> peers(G.world);
+    for (int r = 0; r < G.world; ++r) {
+        GroupSlabBlob b;
+        memcpy(&b, all.data() + (size_t)r * sizeof(GroupSlabBlob), sizeof(b));
+        if (!b.ok) {
+            for (GroupRank* x : G.ranks)
+                x->release();
+            throw CudaError(b.error[0] ? std::string(b.error) : "group: rank " + std::to_string(r) + " could not take its share");
+        }
+        peers[r] = b.slab;
+    }
+    // C: map the peers' mailboxes
+    for (size_t i = 0; i < nr; ++i)
+        G.ranks[i]->map_peers(peers.data());
+    std::vector<std::vector<uint8_t>> tick(nr, std::vector<uint8_t>(4, 0));
+    G.exchange(tick, all, 4); // nobody searches before everybody has mapped everybody
+    G.root = root;
+    G.distributed = true;
+}
+
+void group_rank_info(Group& G, int which, lb200_group_rank_info_t& out) {
+    std::lock_guard<std::mutex> lk(G.mu);
+    if (which < 0 || (size_t)which >= G.ranks.size())
+        throw CudaError("group: no such local rank");
+    if (!G.distributed)
+        throw CudaError("group: lb200_group_distribute or lb200_group_load has not been called");
+    G.ranks[which]->footprint(out);
 }
 
 // A temporary copy of `root` on the current device for a group build: the root's config, codebook and PQ tables, its rows

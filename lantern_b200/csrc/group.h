@@ -59,6 +59,10 @@ void group_free(Group* G);
 int group_world(const Group& G);
 int group_local_ranks(const Group& G);
 void group_distribute(Group& G, Index* root_index, int root, size_t max_batch, size_t max_results);
+// the same distribution from the bytes of an index file that every rank passes; `cfg` plays the part of the index's options
+void group_load(Group& G, const IndexConfig& cfg, const void* buffer, size_t length, int root, size_t max_batch,
+                size_t max_results);
+void group_rank_info(Group& G, int which, lb200_group_rank_info_t& out);
 void group_build(Group& G, Index* root_index, int root);
 void group_search_device(Group& G, const void* d_queries, size_t nq, size_t stride, int kind, size_t k, size_t ef,
                          uint64_t* d_keys, float* d_dists, uint32_t* d_counts, cudaStream_t stream);
