@@ -338,7 +338,7 @@ struct ora_index {
     uint32_t* visit;
     uint32_t epoch;
     uint32_t rng; /* std::default_random_engine == minstd_rand0, default seed 1 */
-    int engine_order; /* 0 = the reference's heap; 1 = the CUDA engine's tie order (search only) */
+    int engine_order; /* 0 = the reference's heap; 1 = the CUDA engine's tie order (search and insertion beams) */
     float *dec_a, *dec_b;
     uint8_t* cast_buf;
     ora_stats st;
@@ -523,12 +523,15 @@ static void search_base(ora_index* x, const void* q, uint32_t start, size_t top_
     }
 }
 
-/* The same beam with the CUDA engine's queue discipline (lantern_b200/csrc/walk.cuh beam_impl): the candidate queue is the
- * set of unexpanded entries of `top` (closest first; among equal distances the most recently inserted first, which is what
- * insert-before-equal gives) plus a LIFO "limbo" of unexpanded entries evicted at exactly the current radius.  Identical to
- * search_base whenever no two candidate distances are exactly equal; with ties only the ORDER of equal-distance expansions
- * differs from the reference's binary heap.  Used to show that ties are the only source of id differences. */
-static void search_base_engine_order(ora_index* x, const void* q, uint32_t start, size_t top_limit) {
+/* The beam of search_base / search_to_insert with the CUDA engine's queue discipline (lantern_b200/csrc/walk.cuh
+ * beam_impl), for search (level 0, skip == UINT32_MAX) and for insertion (level l, skip == the new node) alike: the
+ * candidate queue is the set of unexpanded entries of `top` (closest first; among equal distances the most recently
+ * inserted first, which is what insert-before-equal gives) plus a LIFO "limbo" of unexpanded entries evicted at exactly
+ * the current radius (at most 64, walk.cuh kLimboCap; dropped when the radius shrinks below them).  A popped `skip` is
+ * not expanded (index.hpp:3357; beam_impl's `c == skip`).  Identical to the heap beams whenever no two candidate
+ * distances are exactly equal; with ties only the ORDER of equal-distance expansions differs from the reference's binary
+ * heap, and then this order is the engine's: its searches and its builds are pinned against this function. */
+static void beam_engine_order(ora_index* x, const void* q, uint32_t start, uint32_t skip, int level, size_t top_limit) {
     cvec_t* top = &x->top;
     uint8_t* expanded = (uint8_t*)calloc(top_limit + 1, 1);
     uint32_t limbo[64];
@@ -551,9 +554,13 @@ static void search_base_engine_order(ora_index* x, const void* q, uint32_t start
             c = limbo[--limbo_n];
         if (c == UINT32_MAX)
             break;
-        x->st.base_pops++;
-        uint32_t n = x->cnt0[c], j;
-        const uint32_t* l = x->nbr0 + (size_t)c * x->M0;
+        if (c == skip)
+            continue;
+        if (skip == UINT32_MAX) /* search: counted like search_base */
+            x->st.base_pops++;
+        uint32_t* cnt;
+        const uint32_t* l = nbr_list(x, c, level, &cnt);
+        uint32_t n = *cnt, j;
         for (j = 0; j < n; ++j) {
             uint32_t s = l[j];
             if (visits_set(x, s))
@@ -583,9 +590,13 @@ static void search_base_engine_order(ora_index* x, const void* q, uint32_t start
     free(expanded);
 }
 
-/* search_to_insert_, index.hpp:3324-3392. */
+/* search_to_insert_, index.hpp:3324-3392 (engine_order: the engine's tie order, beam_engine_order). */
 static void search_to_insert(ora_index* x, const void* q, uint32_t start, uint32_t new_slot, int level,
                              size_t top_limit) {
+    if (x->engine_order) {
+        beam_engine_order(x, q, start, new_slot, level, top_limit);
+        return;
+    }
     cvec_t *next = &x->next, *top = &x->top;
     visits_clear(x);
     next->n = 0, top->n = 0;
@@ -764,8 +775,8 @@ int ora_add(ora_index* x, uint64_t key, const void* vector, int kind, int level,
  * Model of the CUDA engine's BATCHED build (lantern_b200/csrc/build.cu) -- not a reference function.
  * The reference inserts one node at a time; the engine inserts batches in two phases so that thousands of inserts
  * run concurrently.  This restates that schedule on top of the reference procedures above, so that the engine's
- * default build can be checked bit for bit against a CPU specification (tests/test_gpu_build.py) instead of only
- * statistically (recall):
+ * default build can be checked bit for bit against a CPU specification (tests/test_gpu_build_model.py, with engine_order on
+ * so that the insertion beams break distance ties as the engine does) instead of only statistically (recall):
  *   levels are drawn up front for all pending vectors (same generator, same order as sequential inserts);
  *   a batch holds min(remaining, batch_cap, max(1, visible / build_ratio)) nodes and is cut in front of a node whose
  *   level exceeds the current top level (such a node is inserted alone and then becomes the entry point);
@@ -947,7 +958,7 @@ size_t ora_search(ora_index* x, const void* query, int kind, size_t k, size_t ef
         expansion = k;
     uint32_t closest = search_for_one(x, q, (uint32_t)x->entry, x->max_level, 0);
     if (x->engine_order)
-        search_base_engine_order(x, q, closest, expansion);
+        beam_engine_order(x, q, closest, UINT32_MAX, 0, expansion);
     else
         search_base(x, q, closest, expansion);
     size_t found = x->top.n < k ? x->top.n : k, i;

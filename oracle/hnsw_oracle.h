@@ -37,8 +37,8 @@ ora_index* ora_init(int metric, int quant, size_t dims, size_t connectivity, siz
 void ora_free(ora_index*);
 int ora_reserve(ora_index*, size_t capacity);
 size_t ora_size(const ora_index*);
-/* 1: base-layer search pops equal-distance candidates in the CUDA engine's order instead of the reference heap's (results are
- * identical on tie-free data; see search_base_engine_order). */
+/* 1: the base-layer search and the insertion beams (ora_add, ora_add_batch_engine) pop equal-distance candidates in the CUDA
+ * engine's order instead of the reference heap's (results are identical on tie-free data; see beam_engine_order). */
 void ora_set_engine_order(ora_index*, int on);
 size_t ora_dimensions(const ora_index*);
 size_t ora_connectivity(const ora_index*);

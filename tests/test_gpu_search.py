@@ -81,7 +81,7 @@ def test_hamming_bits(eng, port):
     # heavy ties: against the reference's heap order only the distance profile is comparable ...
     assert np.array_equal(gd[:, 0], pd[:, 0])
     assert np.mean(gd == pd) > 0.98
-    # ... but against the oracle run with the engine's own tie order (hnsw_oracle.c search_base_engine_order) the ids are
+    # ... but against the oracle run with the engine's own tie order (hnsw_oracle.c beam_engine_order) the ids are
     # IDENTICAL: exact distance ties are the only reason ids ever differ from the reference
     p.set_engine_order(True)
     ek, ed, _, etot = p.search_batch(Q, 10)

@@ -206,6 +206,58 @@ def test_batched_build_model_with_batches_of_one_is_sequential_insertion(port, m
     assert np.array_equal(a.save_buffer(), b.save_buffer())
 
 
+def _model_file(port, X, dim, metric, quant, M, efc, batch, engine_order):
+    keys = np.arange(1, len(X) + 1, dtype=np.uint64)
+    p = port.PortIndex(dim, metric, quant, M=M, efc=efc, ef=32)
+    p.set_engine_order(engine_order)
+    p.reserve(len(X))
+    p.add_batch_engine(keys, X, batch, 64)
+    return p.save_buffer()
+
+
+@pytest.mark.parametrize("batch", [1, 64])
+@pytest.mark.parametrize("M", [4, 16])
+@pytest.mark.parametrize("metric", ["l2sq", "cos"])
+def test_engine_order_build_equals_heap_order_without_ties(port, metric, M, batch):
+    """On float data without exact distance ties the engine's tie order (set before adding: it then governs the insertion
+    beams too) changes nothing: the same file, byte for byte, as the reference's heap order."""
+    from util import structured
+    X = structured(1500, 24, seed=31)
+    a = _model_file(port, X, 24, metric, "f32", M, 64, batch, False)
+    b = _model_file(port, X, 24, metric, "f32", M, 64, batch, True)
+    assert np.array_equal(a, b)
+
+
+@pytest.mark.parametrize("batch", [1, 64])
+def test_engine_order_reaches_the_insertion_beam(port, batch):
+    """Clustered hamming data, where exact ties are everywhere: the two orders build different graphs (about 30 % of the
+    lists differ), so the switch really reaches search_to_insert and not only the search."""
+    from util import adjacency_lists, hamming_rows
+    X = hamming_rows(2000, 768, seed=1)
+    a = _model_file(port, X, 768, "hamming", "b1", 16, 128, batch, False)
+    b = _model_file(port, X, 768, "hamming", "b1", 16, 128, batch, True)
+    la, _ = adjacency_lists(a, 16, 96)
+    lb, _ = adjacency_lists(b, 16, 96)
+    assert sum(la[k] != lb[k] for k in la) > 0.1 * len(la)
+
+
+@pytest.mark.parametrize("metric,quant", [("l2sq", "f32"), ("cos", "f32"), ("hamming", "b1")])
+def test_engine_order_batches_of_one_are_sequential_insertion(port, metric, quant):
+    """In the engine's tie order too, the batched-build model with batch_cap = 1 is add() node after node."""
+    from util import hamming_rows
+    n = 1500
+    if quant == "b1":
+        X, dim = hamming_rows(n, 192, seed=2), 192
+    else:
+        X, dim = np.random.default_rng(37).integers(-8, 9, (n, 24)).astype(np.float32), 24
+    a = port.PortIndex(dim, metric, quant, M=8, efc=48, ef=32)
+    a.set_engine_order(True)
+    a.reserve(n)
+    for k, v in enumerate(X):
+        a.add(k + 1, v)
+    assert np.array_equal(a.save_buffer(), _model_file(port, X, dim, metric, quant, 8, 48, 1, True))
+
+
 def test_batched_build_model_is_deterministic_and_as_good_as_sequential(port):
     rng = np.random.default_rng(29)
     n, d = 4000, 24

@@ -10,6 +10,26 @@ def structured(n, d, seed, latent=32, noise=0.05):
     return (z @ P + noise * rng.standard_normal((n, d)).astype(np.float32)).astype(np.float32)
 
 
+EXACT_FP32 = 1 << 24  # every integer of magnitude <= 2^24 is an fp32 value: sums of such integers are exact in any order
+
+
+def exact_int_rows(rng, n, d, r, metric):
+    """Integer coordinates in [-r, r] whose distances are exact in fp32 whatever the summation order: every product and
+    every partial sum is an integer below 2^24 (l2sq: d (2r)^2; cos: d r^2 for a.b, |a|^2 and |b|^2)."""
+    bound = d * (2 * r) ** 2 if metric == "l2sq" else d * r * r
+    assert bound < EXACT_FP32, (metric, d, r, bound)
+    return rng.integers(-r, r + 1, (n, d)).astype(np.float32)
+
+
+def hamming_rows(n, bits, seed, protos_seed=5, flip=0.1):
+    """Clustered packed bits (16 random prototypes, each bit flipped with probability `flip`): exact ties everywhere.
+    Bits past `bits` in the last byte are zero."""
+    protos = np.random.default_rng(protos_seed).random((16, bits)) < 0.5
+    r = np.random.default_rng(seed)
+    rows = protos[r.integers(0, 16, n)] ^ (r.random((n, bits)) < flip)
+    return np.packbits(rows, axis=1)
+
+
 def build_port_index(portlib, X, metric="l2sq", quant="f32", M=16, efc=128, ef=64, keys=None, **kw):
     n = len(X)
     dim = X.shape[1] * 8 if X.dtype == np.uint8 else X.shape[1]
@@ -80,11 +100,42 @@ def adjacency_lists(buf, M, stored_bytes):
     return lists, levels
 
 
-def graph_agreement(buf_a, buf_b, M, stored_bytes):
-    """Fraction of (node, level) adjacency lists that are identical (same ids, same order) in two index files."""
-    la, lva = adjacency_lists(buf_a, M, stored_bytes)
-    lb, lvb = adjacency_lists(buf_b, M, stored_bytes)
-    assert np.array_equal(lva, lvb), "level draws differ"
-    assert la.keys() == lb.keys()
-    same = sum(1 for k in la if la[k] == lb[k])
-    return same / max(1, len(la))
+def distance64(a, b, metric, quant):
+    """Distance of two storage-domain rows (f32, f16 as uint16 bits, i8, b1 packed bytes) in float64."""
+    if quant == "b1":
+        return float(np.unpackbits(np.bitwise_xor(a, b)).sum())
+    a = (a.view(np.float16) if quant == "f16" else a).astype(np.float64)
+    b = (b.view(np.float16) if quant == "f16" else b).astype(np.float64)
+    if metric == "l2sq":
+        return float(((a - b) ** 2).sum())
+    a2, b2 = float(a @ a), float(b @ b)
+    if a2 == 0 and b2 == 0:
+        return 0.0
+    if a2 == 0 or b2 == 0:
+        return 1.0
+    return 1.0 - float(a @ b) / (np.sqrt(a2) * np.sqrt(b2))
+
+
+def describe_file_difference(buf_a, buf_b, M, stored_bytes, rows, metric, quant, dims, port, names=("gpu", "model")):
+    """Where two index files of the same rows differ, in terms a person can debug from: the first differing (node, level)
+    adjacency list of each file, and for every id in either list its distance to the node in float64 and by the oracle's
+    fp32 metric.  Equal distances in a different order point at tie order; different distances at the kernel."""
+    a, b = np.asarray(buf_a, np.uint8), np.asarray(buf_b, np.uint8)
+    if len(a) != len(b):
+        return "file lengths differ: %s %d bytes, %s %d bytes" % (names[0], len(a), names[1], len(b))
+    la, lva = adjacency_lists(a, M, stored_bytes)
+    lb, lvb = adjacency_lists(b, M, stored_bytes)
+    if not np.array_equal(lva, lvb):
+        return "level draws differ, first at node %d" % int(np.nonzero(lva != lvb)[0][0])
+    differ = [k for k in sorted(la) if la[k] != lb[k]]
+    if not differ:
+        return "adjacency lists identical; first differing byte at offset %d" % int(np.nonzero(a != b)[0][0])
+    node, level = differ[0]
+    out = ["%d of %d adjacency lists differ; first at node %d, level %d" % (len(differ), len(la), node, level),
+           "  %-5s %s" % (names[0], list(la[(node, level)])), "  %-5s %s" % (names[1], list(lb[(node, level)]))]
+    ids = sorted(set(la[(node, level)]) | set(lb[(node, level)]), key=lambda i: (distance64(rows[node], rows[i], metric, quant), i))
+    for i in ids:
+        out.append("  id %6d  float64 %-22.17g oracle fp32 %-14.9g in %s" % (
+            i, distance64(rows[node], rows[i], metric, quant), port.distance(rows[node], rows[i], metric, quant, dims),
+            "+".join(n for n, l in zip(names, (la, lb)) if i in l[(node, level)]) or "-"))
+    return "\n".join(out)
