@@ -318,11 +318,13 @@ LB200_EXPORT void lb200_merge_shards_device(lb200_key_t const* d_keys, lb200_dis
  *                             (every rank passes `bytes_per_rank` bytes, everybody receives world * bytes_per_rank, rank
  *                             order); it is used at creation/distribution time only, never on the search path;
  *   lb200_group_create_local  one process driving n devices (what a Lantern indexing/search server would do).
- * and two ways to give it its graph (once per group):
+ * and three ways to give it its graph (once per group):
  *   lb200_group_distribute    the root rank passes a built (or loaded) index that lives on ITS device; every rank copies its
  *                             row range and the graph from it over NVLink.  The index must fit on one GPU.
  *   lb200_group_load[_buffer] every rank reads its row range and the graph straight from an index file; no GPU ever holds
  *                             all rows, so the group can serve an index larger than one GPU.
+ *   lb200_group_index_init    the group gets an empty index of its own, fills it with lb200_group_index_add_batch and builds
+ *                             it with all ranks (lb200_group_index_build); no GPU ever holds all rows here either.
  * lb200_group_search_batch*: collective; only the root's queries are read (other ranks may pass NULL); EVERY rank receives
  * the full result (the final all-gather is fused into the kernel's epilogue: owners store their top-k into every rank). */
 typedef void* lb200_group_t;
@@ -379,6 +381,34 @@ LB200_EXPORT void lb200_group_rank_info(lb200_group_t, int local_rank, lb200_gro
  * default (0) is the one-GPU default times the number of ranks.  The group's distribution is not touched: call
  * lb200_group_distribute afterwards to search the new graph on the group.  Refused for multi-process groups. */
 LB200_EXPORT void lb200_group_build(lb200_group_t, lb200_index_t root_index, int root, lb200_error_t* error);
+/* ---- the group's own index (single-process groups): built straight into the row-sharded layout, then searched and saved ----
+ * lb200_group_index_init: the group gets an empty index with `options` (as lb200_init reads them) and room for `capacity`
+ * rows.  Rank r holds rows [capacity r / G, capacity (r+1) / G) for the life of the group; lists and keys of all `capacity`
+ * rows are kept on every rank.  max_batch / max_results: as in lb200_group_distribute.  PQ options are refused (a group
+ * cannot hold PQ codes), and so are multi-process groups.  A group takes one lb200_group_distribute, lb200_group_load or
+ * lb200_group_index_init, never two.  lb200_group_search_batch* and lb200_group_rank_info then work on this index; rank_info
+ * reports each rank's capacity range and bytes_rows for that range.  Pending rows are built by the next save or search, as
+ * with a one-GPU index. */
+LB200_EXPORT void lb200_group_index_init(lb200_group_t, lb200_init_options_t const* options, size_t capacity, size_t max_batch,
+                                         size_t max_results, lb200_error_t* error);
+/* Host rows, f32 or packed b1, with the input and key checks of lb200_add_batch.  Row i of the index goes only to the rank whose
+ * range holds it, cast to the storage kind there, through a bounded pinned block.  Adding past `capacity` is refused and adds
+ * nothing. */
+LB200_EXPORT void lb200_group_index_add_batch(lb200_group_t, lb200_key_t const* keys, void const* vectors, size_t n, size_t stride,
+                                              lb200_scalar_kind_t kind, lb200_error_t* error);
+/* "build_batch" and "build_ratio", as lb200_set_option; the default batch cap is the one-GPU default times the ranks. */
+LB200_EXPORT void lb200_group_index_set_option(lb200_group_t, char const* name, size_t value, lb200_error_t* error);
+/* Inserts every pending row with all ranks: the graph lb200_build makes on one GPU with the same rows and batch cap. */
+LB200_EXPORT void lb200_group_index_build(lb200_group_t, lb200_error_t* error);
+/* as lb200_size / lb200_last_build_stats of a one-GPU index */
+LB200_EXPORT size_t lb200_group_index_size(lb200_group_t, lb200_error_t* error);
+LB200_EXPORT void lb200_group_index_last_build_stats(lb200_group_t, lb200_build_stats_t* stats, lb200_error_t* error);
+/* The usearch/lantern file, as lb200_serialized_length / lb200_save_buffer / lb200_save.  The graph comes from rank 0 and the
+ * rows from each rank in turn through a bounded host block: no host buffer holds all rows, and lb200_group_index_save streams
+ * the file to disk. */
+LB200_EXPORT size_t lb200_group_index_serialized_length(lb200_group_t, lb200_error_t* error);
+LB200_EXPORT void lb200_group_index_save_buffer(lb200_group_t, void* buffer, size_t length, lb200_error_t* error);
+LB200_EXPORT void lb200_group_index_save(lb200_group_t, char const* path, lb200_error_t* error);
 /* host buffers in and out (host<->device copies included); counts may be NULL */
 LB200_EXPORT void lb200_group_search_batch(lb200_group_t, void const* queries, size_t nq, size_t stride,
                                            lb200_scalar_kind_t query_kind, size_t count, size_t ef, lb200_key_t* keys,

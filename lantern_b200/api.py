@@ -162,6 +162,15 @@ SIGNATURES = {
     "lb200_group_load": (None, [C.c_void_p, C.POINTER(InitOptions), C.c_char_p, C.c_int, C.c_size_t, C.c_size_t, ERRP]),
     "lb200_group_rank_info": (None, [C.c_void_p, C.c_int, C.POINTER(GroupRankInfo), ERRP]),
     "lb200_group_build": (None, [C.c_void_p, C.c_void_p, C.c_int, ERRP]),
+    "lb200_group_index_init": (None, [C.c_void_p, C.POINTER(InitOptions), C.c_size_t, C.c_size_t, C.c_size_t, ERRP]),
+    "lb200_group_index_add_batch": (None, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, ERRP]),
+    "lb200_group_index_set_option": (None, [C.c_void_p, C.c_char_p, C.c_size_t, ERRP]),
+    "lb200_group_index_build": (None, [C.c_void_p, ERRP]),
+    "lb200_group_index_size": (C.c_size_t, [C.c_void_p, ERRP]),
+    "lb200_group_index_last_build_stats": (None, [C.c_void_p, C.POINTER(BuildStats), ERRP]),
+    "lb200_group_index_serialized_length": (C.c_size_t, [C.c_void_p, ERRP]),
+    "lb200_group_index_save_buffer": (None, [C.c_void_p, C.c_void_p, C.c_size_t, ERRP]),
+    "lb200_group_index_save": (None, [C.c_void_p, C.c_char_p, ERRP]),
     "lb200_group_search_batch": (None, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_size_t, C.c_size_t,
                                         C.c_void_p, C.c_void_p, C.c_void_p, ERRP]),
     "lb200_group_search_batch_device": (None, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_size_t, C.c_size_t,
@@ -355,6 +364,7 @@ class Group:
     Group.ranked(rank, world, ag)   one process per GPU; `ag(send: bytes) -> bytes` is the caller's all-gather
                                     (concatenation of every rank's `send`, rank order), used for bootstrap only
     then once: distribute(index) (an index on the root's GPU) or load(path) / load_buffer(bytes) (each rank reads its rows)
+               or index_init(capacity, ...) (an index of the group's own: index_add_batch, index_build, index_save)
     """
 
     def __init__(self, handle, world, keep=None):
@@ -436,6 +446,41 @@ class Group:
     def build(self, index, root=0):
         """Insert every pending vector of `index` (on rank `root`'s device) with all ranks: lb200_build's graph, byte for byte."""
         self._call("lb200_group_build", index.h if index is not None else None, root)
+
+    # ---- the group's own index (lb200_group_index_*): built straight into the row-sharded layout ----
+    def index_init(self, capacity, dim, metric="l2sq", quant="f32", M=16, efc=128, ef=64, pq=False, max_batch=8192,
+                   max_results=0):
+        """An empty index of the group's own with room for `capacity` rows; rank r holds rows [capacity r / G, capacity (r+1) / G)."""
+        o = init_options(dim, metric, quant, M, efc, ef, pq)
+        self._call("lb200_group_index_init", C.byref(o), capacity, max_batch, max_results)
+
+    def index_add_batch(self, keys, vecs):
+        vecs = np.ascontiguousarray(vecs)
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        self._call("lb200_group_index_add_batch", _ptr(keys), _ptr(vecs), len(keys), vecs.strides[0], Index._kind(vecs))
+
+    def index_set_option(self, name, value):
+        self._call("lb200_group_index_set_option", name.encode(), int(value))
+
+    def index_build(self):
+        self._call("lb200_group_index_build")
+
+    def index_size(self):
+        return self._call("lb200_group_index_size")
+
+    def index_last_build_stats(self):
+        s = BuildStats()
+        self._call("lb200_group_index_last_build_stats", C.byref(s))
+        return {f: getattr(s, f) for f, _ in BuildStats._fields_}
+
+    def index_save_buffer(self):
+        n = self._call("lb200_group_index_serialized_length")
+        buf = np.zeros(n, np.uint8)
+        self._call("lb200_group_index_save_buffer", _ptr(buf), n)
+        return buf
+
+    def index_save(self, path):
+        self._call("lb200_group_index_save", path.encode())
 
     def search_batch(self, queries, k, ef=0, nq=None, dim_bytes=None, kind=None):
         """Host buffers.  Non-root ranks of a multi-process group pass queries=None with nq / dim_bytes / kind."""

@@ -24,6 +24,10 @@
 // rank r applies the segments seg = r (mod G).  The replicated kernels (REP = true) store every list and every request
 // into all replicas over NVLink, so that each phase stays one launch per rank.  The result is the one-GPU graph, byte for
 // byte: no step depends on which CTA, or which GPU, does the work.
+//
+// Row-sharded group build (lb200_group_index_build): the same schedule and phases, but rank r's index holds only the rows of
+// its range; the replicated kernels' TABLE instantiation reads every row, the new node's own included, through a per-launch
+// table of the ranks' row arrays (RowTable, walk.cuh).
 #include <cuda_runtime.h>
 
 #include <cub/cub.cuh>
@@ -45,7 +49,7 @@ struct BuildLaunch {
     uint32_t* upper_adj;
     uint32_t u0, count;        // batch = nodes [u0, u0 + count)
     const int32_t* new_levels; // [count]
-    const uint8_t* values;     // value (query side) of batch item i at values + i * value_stride
+    const uint8_t* values;     // value (query side) of batch item i at values + i * value_stride; NULL = node u's row in `rows`
     size_t value_stride;
     uint32_t efc;
     uint32_t top_cap;
@@ -67,13 +71,19 @@ struct BuildLaunch {
     uint32_t* rep_upper_adj[kGroupMax];
     unsigned long long* rep_req_keys[kGroupMax];
     unsigned long long* rep_req_vals[kGroupMax];
+    RowTable rows; // row-sharded group build (TABLE = true): where every row lives (walk.cuh)
 };
+static_assert(kGroupMax <= (int)kRowRangesMax, "one row range per rank");
 
-template <class W, bool REP>
+template <class W0, bool REP, bool TABLE = false>
 __global__ void __launch_bounds__(kWalkThreads) build_insert_kernel(const __grid_constant__ BuildLaunch p, const uint32_t R) {
+    static_assert(REP || !TABLE, "the row table serves the replicated kernels only");
+    using W = std::conditional_t<TABLE, typename RowTableWalker<W0>::type, W0>;
     extern __shared__ __align__(128) uint8_t smem_raw[];
     const WalkLayout lay = W::layout(p.g, R, p.top_cap, p.g.M0 + 1);
     W w(p.g);
+    if constexpr (W::kRowTable)
+        w.rows = &p.rows;
     w.init(smem_raw, lay, R, p.s);
     WalkSmem& sm = w.sm;
     const uint32_t M = p.g.M, M0 = p.g.M0;
@@ -88,7 +98,11 @@ __global__ void __launch_bounds__(kWalkThreads) build_insert_kernel(const __grid
             break;
         const uint32_t u = p.u0 + item;
         const int lu = p.new_levels[item];
-        const uint8_t* urow = p.values + (size_t)item * p.value_stride;
+        const uint8_t* urow;
+        if constexpr (W::kRowTable)
+            urow = p.values ? p.values + (size_t)item * p.value_stride : w.row_addr(u);
+        else
+            urow = p.values + (size_t)item * p.value_stride;
         w.load_value(urow);
 
         uint32_t cur = p.g.entry;
@@ -158,12 +172,16 @@ struct SegmentHead {
     }
 };
 
-template <class W, bool REP>
+template <class W0, bool REP, bool TABLE = false>
 __global__ void __launch_bounds__(kWalkThreads) build_reverse_kernel(const __grid_constant__ BuildLaunch p, const uint32_t R) {
+    static_assert(REP || !TABLE, "the row table serves the replicated kernels only");
+    using W = std::conditional_t<TABLE, typename RowTableWalker<W0>::type, W0>;
     extern __shared__ __align__(128) uint8_t smem_raw[];
     const uint32_t M = p.g.M, M0 = p.g.M0;
     const WalkLayout lay = W::layout(p.g, R, M0 + 2, M0 + 1);
     W w(p.g);
+    if constexpr (W::kRowTable)
+        w.rows = &p.rows;
     w.init(smem_raw, lay, R, p.s);
     WalkSmem& sm = w.sm;
     uint32_t* lst_i = reinterpret_cast<uint32_t*>(smem_raw + lay.total);
@@ -377,6 +395,8 @@ void build_pending_group(Index& idx, const std::vector<BuildReplica>& replicas, 
 }
 
 void build_pending(Index& idx) {
+    if (idx.sharded_)
+        throw CudaError("build: this index's rows are spread over a group; build it with lb200_group_index_build");
     int dev = 0;
     LB_CUDA(cudaGetDevice(&dev));
     build_pending_group(idx, std::vector<BuildReplica>(1, BuildReplica{&idx, dev}), 0);
@@ -395,6 +415,18 @@ static void build_pending_impl(Index& idx, const std::vector<BuildReplica>& repl
     const bool group = G > 1;
     if (G < 1 || G > (uint32_t)kGroupMax || root < 0 || (uint32_t)root >= G || replicas[root].idx != &idx)
         throw CudaError("build: bad rank layout");
+    // row-sharded (a group's own index, group.cu): rank r's index holds rows [row_lo_, row_hi_) only, the ranks' ranges tile
+    // [0, capacity) in rank order, and the replicated kernels read every row through the ranks' table
+    const bool sharded = idx.sharded_;
+    if (sharded) {
+        if (cfg.pq)
+            throw CudaError("build: a row-sharded index cannot hold pq codes");
+        for (uint32_t r = 0; r < G; ++r)
+            if (!replicas[r].idx->sharded_ || replicas[r].idx->row_lo_ != (r ? replicas[r - 1].idx->row_hi_ : 0))
+                throw CudaError("build: the ranks' row ranges do not tile the index");
+        if (replicas[G - 1].idx->row_hi_ < n0 + P)
+            throw CudaError("build: pending rows beyond the ranks' row ranges");
+    }
 
     // ---- levels + upper-list allocation for the new nodes ----
     idx.h_levels_.resize(n0 + P);
@@ -446,8 +478,15 @@ static void build_pending_impl(Index& idx, const std::vector<BuildReplica>& repl
                 occ_ins = occupancy(build_insert_kernel<W, false>, smem_ins);
                 occ_rev = occupancy(build_reverse_kernel<W, false>, smem_rev);
             }
-            grid_ins[r] = sms * (group ? occupancy(build_insert_kernel<W, true>, smem_ins) : occ_ins);
-            grid_rev[r] = sms * (group ? occupancy(build_reverse_kernel<W, true>, smem_rev) : occ_rev);
+            if (!group) {
+                grid_ins[r] = sms * occ_ins, grid_rev[r] = sms * occ_rev;
+            } else if (!sharded) {
+                grid_ins[r] = sms * occupancy(build_insert_kernel<W, true>, smem_ins);
+                grid_rev[r] = sms * occupancy(build_reverse_kernel<W, true>, smem_rev);
+            } else if constexpr (W::kTableWalker) {
+                grid_ins[r] = sms * occupancy(build_insert_kernel<W, true, true>, smem_ins);
+                grid_rev[r] = sms * occupancy(build_reverse_kernel<W, true, true>, smem_rev);
+            }
         });
         b.idx->ensure_scratch(std::max(grid_ins[r], grid_rev[r]));
         if (group) {
@@ -522,6 +561,9 @@ static void build_pending_impl(Index& idx, const std::vector<BuildReplica>& repl
             if (cfg.pq) { // value = the raw f32 vector; stored side = codes
                 q.value_stride = round_up(cfg.dims * 4, 16);
                 q.values = (const uint8_t*)x.d_pending_raw_ + (pos + s0) * q.value_stride;
+            } else if (sharded && group) { // the new node's row may live on any rank: read it through the table
+                q.value_stride = row_bytes;
+                q.values = nullptr;
             } else {
                 q.value_stride = row_bytes;
                 q.values = x.d_vectors_ + (size_t)q.u0 * row_bytes;
@@ -538,6 +580,11 @@ static void build_pending_impl(Index& idx, const std::vector<BuildReplica>& repl
                 q.rep_adj0[t] = rk[t].idx->d_adj0_, q.rep_upper_adj[t] = rk[t].idx->d_upper_adj_;
                 q.rep_req_keys[t] = rk[t].req_keys.p + s0 * req_stride, q.rep_req_vals[t] = rk[t].req_vals.p + s0 * req_stride;
             }
+            if (sharded) { // every rank's slice: its own, and its peers' through peer mappings (one process, UVA pointers)
+                q.rows.count = G, q.rows.own = r;
+                for (uint32_t t = 0; t < G; ++t)
+                    q.rows.hi[t] = (uint32_t)rk[t].idx->row_hi_, q.rows.base[t] = rk[t].idx->d_vectors_;
+            }
         }
         // phase 1: rank r inserts its slice
         for (uint32_t r = 0; r < G; ++r) {
@@ -553,10 +600,12 @@ static void build_pending_impl(Index& idx, const std::vector<BuildReplica>& repl
             if (grid) {
                 dispatch_walker(cfg.pq, idx.dist_mode_, cfg.scalar_kind, nq, [&](auto tag) {
                     using W = typename decltype(tag)::type;
-                    if (group)
-                        build_insert_kernel<W, true><<<grid, kWalkThreads, smem_ins, b.stream>>>(p[r], R);
-                    else
+                    if (!group)
                         build_insert_kernel<W, false><<<grid, kWalkThreads, smem_ins, b.stream>>>(p[r], R);
+                    else if (!sharded)
+                        build_insert_kernel<W, true><<<grid, kWalkThreads, smem_ins, b.stream>>>(p[r], R);
+                    else if constexpr (W::kTableWalker)
+                        build_insert_kernel<W, true, true><<<grid, kWalkThreads, smem_ins, b.stream>>>(p[r], R);
                 });
                 LB_CUDA(cudaGetLastError());
                 count_launch();
@@ -595,10 +644,12 @@ static void build_pending_impl(Index& idx, const std::vector<BuildReplica>& repl
             const uint32_t grid = (uint32_t)std::min<size_t>(nreq, grid_rev[r]);
             dispatch_walker(cfg.pq, idx.dist_mode_, cfg.scalar_kind, nq, [&](auto tag) {
                 using W = typename decltype(tag)::type;
-                if (group)
-                    build_reverse_kernel<W, true><<<grid, kWalkThreads, smem_rev, b.stream>>>(p[r], R);
-                else
+                if (!group)
                     build_reverse_kernel<W, false><<<grid, kWalkThreads, smem_rev, b.stream>>>(p[r], R);
+                else if (!sharded)
+                    build_reverse_kernel<W, true><<<grid, kWalkThreads, smem_rev, b.stream>>>(p[r], R);
+                else if constexpr (W::kTableWalker)
+                    build_reverse_kernel<W, true, true><<<grid, kWalkThreads, smem_rev, b.stream>>>(p[r], R);
             });
             LB_CUDA(cudaGetLastError());
             count_launch();

@@ -910,6 +910,97 @@ LB200_EXPORT void lb200_group_rank_info(lb200_group_t h, int local_rank, lb200_g
 LB200_EXPORT void lb200_group_build(lb200_group_t h, lb200_index_t root_index, int root, lb200_error_t* error) {
     guarded(error, [&] { group_build(*as_group(h), reinterpret_cast<Index*>(root_index), root); });
 }
+LB200_EXPORT void lb200_group_index_init(lb200_group_t h, lb200_init_options_t const* options, size_t capacity, size_t max_batch,
+                                         size_t max_results, lb200_error_t* error) {
+    guarded(error, [&] {
+        Group& G = *as_group(h);
+        const IndexConfig cfg = group_load_config(options);
+        group_index_init(G, cfg, capacity, group_max_batch(max_batch), group_max_results(max_batch, max_results));
+    });
+}
+LB200_EXPORT void lb200_group_index_add_batch(lb200_group_t h, lb200_key_t const* keys, void const* vectors, size_t n, size_t stride,
+                                              lb200_scalar_kind_t kind, lb200_error_t* error) {
+    guarded(error, [&] { group_index_add(*as_group(h), keys, vectors, n, stride, kind); });
+}
+LB200_EXPORT void lb200_group_index_set_option(lb200_group_t h, char const* name, size_t value, lb200_error_t* error) {
+    guarded(error, [&] { group_index_set_option(*as_group(h), name ? name : "", value); });
+}
+LB200_EXPORT void lb200_group_index_build(lb200_group_t h, lb200_error_t* error) {
+    guarded(error, [&] { group_index_build(*as_group(h)); });
+}
+LB200_EXPORT size_t lb200_group_index_size(lb200_group_t h, lb200_error_t* error) {
+    size_t r = 0;
+    guarded(error, [&] { r = group_index_size(*as_group(h)); });
+    return r;
+}
+LB200_EXPORT void lb200_group_index_last_build_stats(lb200_group_t h, lb200_build_stats_t* stats, lb200_error_t* error) {
+    guarded(error, [&] {
+        if (!stats)
+            throw CudaError("null stats pointer");
+        size_t vectors = 0, value_bytes = 0;
+        uint64_t dist = 0;
+        double ms = 0;
+        group_index_build_stats(*as_group(h), vectors, dist, ms, value_bytes);
+        stats->vectors = vectors;
+        stats->computed_distances = dist;
+        stats->algorithmic_bytes = dist * value_bytes;
+        stats->device_ms = ms;
+    });
+}
+LB200_EXPORT size_t lb200_group_index_serialized_length(lb200_group_t h, lb200_error_t* error) {
+    size_t r = 0;
+    guarded(error, [&] { r = group_index_serialized_length(*as_group(h)); });
+    return r;
+}
+LB200_EXPORT void lb200_group_index_save_buffer(lb200_group_t h, void* buffer, size_t length, lb200_error_t* error) {
+    guarded(error, [&] {
+        Group& G = *as_group(h);
+        if (!buffer)
+            throw CudaError("null buffer");
+        uint8_t* p = (uint8_t*)buffer;
+        group_index_save(
+            G,
+            [&](size_t need) {
+                if (length < need)
+                    throw CudaError("save_buffer: buffer too small (see lb200_group_index_serialized_length)");
+            },
+            [&](const void* bytes, size_t n) {
+                memcpy(p, bytes, n);
+                p += n;
+            });
+    });
+}
+LB200_EXPORT void lb200_group_index_save(lb200_group_t h, char const* path, lb200_error_t* error) {
+    guarded(error, [&] {
+        Group& G = *as_group(h);
+        if (!path)
+            throw CudaError("null path");
+        struct File {
+            FILE* f = nullptr;
+            ~File() {
+                if (f)
+                    fclose(f);
+            }
+        } out;
+        bool opened = false;
+        group_index_save(
+            G,
+            [&](size_t) { // (the index is built and its length known before the file is created)
+                out.f = fopen(path, "wb");
+                if (!out.f)
+                    throw CudaError("Can't open file for writing");
+                opened = true;
+            },
+            [&](const void* bytes, size_t n) {
+                if (fwrite(bytes, 1, n, out.f) != n)
+                    throw CudaError("Failed to write the index file");
+            });
+        const int rc = opened ? fclose(out.f) : 0;
+        out.f = nullptr;
+        if (rc != 0)
+            throw CudaError("Failed to write the index file");
+    });
+}
 LB200_EXPORT void lb200_group_search_batch(lb200_group_t h, void const* queries, size_t nq, size_t stride,
                                            lb200_scalar_kind_t kind, size_t count, size_t ef, lb200_key_t* keys,
                                            lb200_distance_t* distances, size_t* counts, lb200_error_t* error) {

@@ -118,6 +118,24 @@ void Index::ensure_capacity(size_t cap) {
     capacity_ = nc;
 }
 
+void Index::init_row_range(size_t capacity, size_t lo, size_t hi) {
+    if (capacity_ || n_ || pending_n_ || cfg_.pq || lo > hi || hi > capacity)
+        throw CudaError("index: a row range needs an empty, non-pq index and lo <= hi <= capacity");
+    sq_bytes_ = 0, sq_on_ = false; // a group's owners do not screen
+    grow_device(d_vectors_, 0, std::max<size_t>(hi - lo, 1) * row_bytes_, 0);
+    grow_device(d_adj0_, 0, capacity * cfg_.M0, 0xFF);
+    grow_device(d_upper_ref_, 0, capacity, 0xFF);
+    grow_device(d_keys_, 0, capacity, 0xFF);
+    capacity_ = capacity;
+    sharded_ = true, row_lo_ = lo, row_hi_ = hi;
+}
+
+void Index::free_scratch() {
+    cudaFree(scratch_.visited), cudaFree(scratch_.touched);
+    scratch_.visited = nullptr, scratch_.touched = nullptr;
+    scratch_.ctas = 0, scratch_.words_per_cta = 0;
+}
+
 void Index::encode_screen(size_t first, size_t count) {
     if (sq_on_)
         launch_sq_encode(d_vectors_ + first * row_bytes_, row_bytes_, count, d_sq_codes_ + first * sq_bytes_, d_sq_meta_ + first, 0);

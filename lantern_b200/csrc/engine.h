@@ -20,6 +20,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <functional>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -173,6 +174,10 @@ class Index {
     // --- used by build.cu / format.cc ---
     void ensure_capacity(size_t cap);
     void alloc_upper(size_t total_lists);
+    // one rank's part of a group's own index (group.cu): d_vectors_ holds rows [lo, hi) only (row i at (i - lo) * row_bytes_);
+    // lists, levels and keys are sized for all `capacity` rows.  No search-screen companion.  Called once, on an empty index.
+    void init_row_range(size_t capacity, size_t lo, size_t hi);
+    void free_scratch(); // the visited bitmaps and touched lists (they grow with capacity x resident CTAs)
 
     IndexConfig cfg_;
     int dist_mode_ = 0;
@@ -180,6 +185,8 @@ class Index {
     size_t vec_bytes_ = 0;    // unpadded bytes of a vector in the metric scalar kind (file format)
     size_t stored_bytes_ = 0; // unpadded bytes kept per node in the file (vec_bytes_ or num_subvectors)
     size_t n_ = 0, capacity_ = 0;
+    bool sharded_ = false;            // init_row_range: this index holds the rows [row_lo_, row_hi_) of a group's index
+    size_t row_lo_ = 0, row_hi_ = 0;
     int32_t max_level_ = -1;
     uint32_t entry_ = 0;
     uint32_t level_rng_ = 1u;   // minstd_rand0 state, default seed (std::default_random_engine, index.hpp:2082)
@@ -364,6 +371,10 @@ struct BuildReplica {
     int device;
 };
 void build_pending_group(Index& idx, const std::vector<BuildReplica>& replicas, int root);
+// format.cu: the file of a row-sharded index, in order, through `write`: header, lists, keys and levels from `graph` (whose
+// device is shards[0]'s), row i from the shard whose [row_lo_, row_hi_) holds it, a bounded block at a time
+using RowShard = BuildReplica;
+void save_row_sharded(Index& graph, const std::vector<RowShard>& shards, const std::function<void(const void*, size_t)>& write);
 // kmeans.cu
 int train_pq_codebook(const float* d_vectors, size_t stride_floats, size_t n, size_t dims, size_t nsub, size_t ncent, bool cosine,
                       size_t max_iter, uint64_t seed, const uint32_t* init_rows, float* d_codebook, cudaStream_t stream);

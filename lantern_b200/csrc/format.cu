@@ -14,6 +14,8 @@
 #include <string.h>
 
 #include <algorithm>
+#include <functional>
+#include <string>
 #include <vector>
 
 #include "engine.h"
@@ -147,6 +149,52 @@ size_t Index::save_buffer(void* buffer, size_t length) {
         p += stored_bytes_;
     }
     return (size_t)(p - (uint8_t*)buffer);
+}
+
+void save_row_sharded(Index& graph, const std::vector<RowShard>& shards, const std::function<void(const void*, size_t)>& write) {
+    const size_t n = graph.n_, M = graph.cfg_.M, M0 = graph.cfg_.M0, row_bytes = graph.row_bytes_, stored = graph.stored_bytes_;
+    if (graph.pending_n_)
+        throw CudaError("save: the index has rows that are not built yet");
+    std::vector<uint32_t> adj0(n * M0), upper_ref(n), upper_adj(graph.upper_lists_ * M);
+    LB_CUDA(cudaSetDevice(shards[0].device));
+    LB_CUDA(cudaDeviceSynchronize());
+    if (n) {
+        LB_CUDA(cudaMemcpy(adj0.data(), graph.d_adj0_, adj0.size() * 4, cudaMemcpyDeviceToHost));
+        LB_CUDA(cudaMemcpy(upper_ref.data(), graph.d_upper_ref_, upper_ref.size() * 4, cudaMemcpyDeviceToHost));
+        if (!upper_adj.empty())
+            LB_CUDA(cudaMemcpy(upper_adj.data(), graph.d_upper_adj_, upper_adj.size() * 4, cudaMemcpyDeviceToHost));
+    }
+    uint8_t head[136];
+    graph.fill_header(head);
+    write(head, sizeof(head));
+    // rows: a block of at most 32 MB at a time, from the rank whose range holds it
+    const size_t block = std::max<size_t>(1, ((size_t)32 << 20) / row_bytes);
+    std::vector<uint8_t> rows(std::min(block, std::max<size_t>(n, 1)) * row_bytes);
+    size_t first = 0, count = 0;
+    std::vector<uint8_t> tape(10 + (4 + 6 * M0) + (size_t)std::max(graph.max_level_, 0) * (4 + 6 * M) + stored);
+    for (size_t i = 0; i < n; ++i) {
+        if (i >= first + count) {
+            size_t t = 0;
+            while (t + 1 < shards.size() && i >= shards[t].idx->row_hi_)
+                ++t;
+            const Index& x = *shards[t].idx;
+            if (i < x.row_lo_ || i >= x.row_hi_)
+                throw CudaError("save: no rank holds row " + std::to_string(i));
+            first = i, count = std::min(std::min(block, x.row_hi_ - i), n - i);
+            LB_CUDA(cudaSetDevice(shards[t].device));
+            LB_CUDA(cudaMemcpy(rows.data(), x.d_vectors_ + (i - x.row_lo_) * row_bytes, count * row_bytes, cudaMemcpyDeviceToHost));
+        }
+        uint8_t* p = tape.data();
+        memcpy(p, &graph.h_keys_[i], 8);
+        memcpy(p + 8, &graph.h_levels_[i], 2);
+        p += 10;
+        p = put_list(p, adj0.data() + i * M0, M0);
+        for (int l = 1; l <= graph.h_levels_[i]; ++l)
+            p = put_list(p, upper_adj.data() + ((size_t)upper_ref[i] + (l - 1)) * M, M);
+        memcpy(p, rows.data() + (i - first) * row_bytes, stored);
+        p += stored;
+        write(tape.data(), (size_t)(p - tape.data()));
+    }
 }
 
 void parse_index_file(const IndexConfig& cfg, size_t vec_bytes, size_t stored_bytes, const void* buffer, size_t length,

@@ -29,9 +29,11 @@
 
 #include <algorithm>
 #include <chrono>
+#include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
+#include <string>
 #include <vector>
 
 #include "../../include/lantern_b200.h"
@@ -1096,6 +1098,10 @@ class GroupRank {
     size_t in_bytes = 0;
     std::vector<uint32_t> h_counts;
     uint32_t h_err = 0;
+    // a group's own index (lb200_group_index_init): rows and graph are those of this rank's Index (borrowed, re-attached after
+    // every build); the rank holds the rows [cap_lo, cap_hi) of an index of `capacity` rows
+    bool borrowed = false;
+    size_t capacity = 0, cap_lo = 0, cap_hi = 0;
 
     ~GroupRank() {
         cudaSetDevice(device);
@@ -1109,8 +1115,11 @@ class GroupRank {
         memset(&f, 0, sizeof(f));
         f.rank = rank, f.world = world;
         f.rows_begin = bounds[rank], f.rows_end = bounds[rank + 1];
+        const size_t g = borrowed ? capacity : n; // a group's own index: sized for its capacity
+        if (borrowed)
+            f.rows_begin = cap_lo, f.rows_end = cap_hi;
         f.bytes_rows = (f.rows_end - f.rows_begin) * row_bytes;
-        f.bytes_graph = n * cfg.M0 * 4 + n * 4 + upper_lists * cfg.M * 4 + n * 8;
+        f.bytes_graph = g * cfg.M0 * 4 + g * 4 + upper_lists * cfg.M * 4 + g * 8;
         f.bytes_scratch = (size_t)Omax * words_per_slot * 4 + (size_t)Omax * touched_cap * 4 + 16 * sizeof(unsigned long long) + in_bytes;
         f.bytes_mailbox = lay.total;
     }
@@ -1118,7 +1127,8 @@ class GroupRank {
     // frees every device allocation of the rank (its peer mappings stay)
     void release() {
         cudaSetDevice(device);
-        cudaFree(d_rows), cudaFree(d_adj0), cudaFree(d_upper_ref), cudaFree(d_upper_adj), cudaFree(d_keys);
+        if (!borrowed)
+            cudaFree(d_rows), cudaFree(d_adj0), cudaFree(d_upper_ref), cudaFree(d_upper_adj), cudaFree(d_keys);
         cudaFree(slab), cudaFree(d_vis), cudaFree(d_touched), cudaFree(d_counters), cudaFree(d_in);
         d_rows = nullptr, d_adj0 = d_upper_ref = d_upper_adj = nullptr, d_keys = nullptr;
         slab = nullptr, d_vis = d_touched = nullptr, d_counters = nullptr, d_in = nullptr;
@@ -1223,7 +1233,7 @@ class GroupRank {
     // may wait for kernels already running on this device, and those kernels wait for the rank that is allocating).  On a
     // failure nothing stays allocated and the error names what did not fit: rows, graph, mailbox or scratch
     // (lb200_group_rank_info_t).
-    void allocate(size_t max_batch_, size_t max_results) {
+    void allocate(size_t max_batch_, size_t max_results, bool graph = true) {
         LB_CUDA(cudaSetDevice(device));
         int sms = 0;
         LB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
@@ -1233,16 +1243,18 @@ class GroupRank {
         // owner slots: one per query a rank owns in the largest batch (never more than the resident warps)
         Omax = (uint32_t)std::min<size_t>(Wmax, round_up((max_batch + world - 1) / world, kGroupWarps));
         lay = slab_layout(Omax, (uint32_t)world, cap, res_cap, max_batch, row_bytes);
-        words_per_slot = round_up((n + 31) / 32, 32); // owner scratch: one visited bitmap per owned slot
+        words_per_slot = round_up((std::max(n, capacity) + 31) / 32, 32); // owner scratch: one visited bitmap per owned slot
         // staging of raw input queries for the host-buffer entry point
         in_bytes = max_batch * std::max<size_t>(row_bytes, cfg.dims * 4);
         const size_t lo = bounds[rank], hi = bounds[rank + 1], owned = Omax;
         try {
-            device_alloc(&d_rows, std::max<size_t>((hi - lo) * row_bytes, 16), "rows");
-            device_alloc(&d_adj0, n * cfg.M0 * 4, "graph (lists, keys)");
-            device_alloc(&d_upper_ref, n * 4, "graph (lists, keys)");
-            device_alloc(&d_upper_adj, std::max<size_t>(upper_lists * cfg.M * 4, 16), "graph (lists, keys)");
-            device_alloc(&d_keys, n * 8, "graph (lists, keys)");
+            if (graph) {
+                device_alloc(&d_rows, std::max<size_t>((hi - lo) * row_bytes, 16), "rows");
+                device_alloc(&d_adj0, n * cfg.M0 * 4, "graph (lists, keys)");
+                device_alloc(&d_upper_ref, n * 4, "graph (lists, keys)");
+                device_alloc(&d_upper_adj, std::max<size_t>(upper_lists * cfg.M * 4, 16), "graph (lists, keys)");
+                device_alloc(&d_keys, n * 8, "graph (lists, keys)");
+            }
             device_alloc(&slab, lay.total, "mailbox");
             device_alloc(&d_vis, owned * words_per_slot * 4, "scratch (visited bitmaps)");
             device_alloc(&d_touched, owned * (size_t)touched_cap * 4, "scratch (touched lists)");
@@ -1292,6 +1304,15 @@ class GroupRank {
             LB_CUDA(cudaMemcpy(d_upper_adj, f.upper_adj.data(), f.upper_adj.size() * 4, cudaMemcpyHostToDevice));
         LB_CUDA(cudaMemcpy(d_keys, f.keys.data(), f.keys.size() * 8, cudaMemcpyHostToDevice));
         LB_CUDA(cudaDeviceSynchronize());
+    }
+
+    // a group's own index: search this rank's Index `x` (its row slice) with the graph state of the root's index.  The search
+    // bounds are min(capacity split, n): trailing ranks may hold no rows yet.
+    void attach(const Index& x, const Index& root) {
+        d_rows = x.d_vectors_, d_adj0 = x.d_adj0_, d_upper_ref = x.d_upper_ref_, d_upper_adj = x.d_upper_adj_, d_keys = x.d_keys_;
+        n = root.n_, upper_lists = root.upper_lists_, entry = root.entry_, max_level = root.max_level_;
+        for (int r = 0; r <= world; ++r)
+            bounds[r] = (uint32_t)std::min(capacity * (size_t)r / (size_t)world, n);
     }
 
     void map_peers(const PtrBlob* slabs) {
@@ -1398,7 +1419,11 @@ struct Group {
     bool distributed = false;
     std::mutex mu;
     std::vector<cudaStream_t> streams; // single-process: one per device
+    // the group's own index (lb200_group_index_init): rank r's Index holds rows [capacity r / G, capacity (r+1) / G); index[0]
+    // also keeps the levels, keys, level generator and batch schedule.  Never handed to the one-GPU entry points.
+    std::vector<std::unique_ptr<Index>> index;
     ~Group() {
+        drop_index();
         for (GroupRank* r : ranks)
             delete r;
         for (size_t i = 0; i < streams.size(); ++i)
@@ -1406,6 +1431,13 @@ struct Group {
                 cudaStreamDestroy(streams[i]);
     }
     bool local() const { return ranks.size() > 1 || world == 1; }
+    void drop_index() { // (each on its own device; the ranks' borrowed pointers go with it)
+        for (size_t i = 0; i < index.size(); ++i) {
+            cudaSetDevice(ranks[i]->device);
+            index[i].reset();
+        }
+        index.clear();
+    }
 
     // every rank contributes `bytes`; everybody receives world * bytes
     void exchange(const std::vector<std::vector<uint8_t>>& mine, std::vector<uint8_t>& all, size_t bytes) {
@@ -1718,6 +1750,218 @@ void group_build(Group& G, Index* root_index, int root) {
     }
 }
 
+// ---- the group's own index (lb200_group_index_*, DESIGN.md 4.2): built straight into the row-sharded layout ---------------
+
+static void require_own_index(Group& G) {
+    if (G.index.empty())
+        throw CudaError("group index: lb200_group_index_init has not been called on this group");
+}
+
+static std::vector<BuildReplica> index_shards(Group& G) {
+    std::vector<BuildReplica> s(G.index.size());
+    for (size_t r = 0; r < s.size(); ++r)
+        s[r] = BuildReplica{G.index[r].get(), G.ranks[r]->device};
+    return s;
+}
+
+void group_index_init(Group& G, const IndexConfig& cfg, size_t capacity, size_t max_batch, size_t max_results) {
+    DeviceGuard dg;
+    std::lock_guard<std::mutex> lk(G.mu);
+    if (G.ranks.size() != (size_t)G.world)
+        throw CudaError("group index: a multi-process group cannot hold an index of its own; create the group with "
+                        "lb200_group_create_local");
+    if (G.distributed)
+        throw CudaError("group index: the group already holds a graph (one lb200_group_distribute, lb200_group_load or "
+                        "lb200_group_index_init per group)");
+    if (cfg.pq)
+        throw CudaError("group index: pq indexes are not supported");
+    if (capacity == 0 || capacity >= 0x7FFFFFFFull)
+        throw CudaError("group index: capacity must be in [1, 2^31 - 1)");
+    const size_t W = (size_t)G.world;
+    try {
+        for (size_t r = 0; r < W; ++r) {
+            GroupRank* gr = G.ranks[r];
+            LB_CUDA(cudaSetDevice(gr->device));
+            G.index.emplace_back(new Index(cfg, nullptr));
+            const size_t lo = capacity * r / W, hi = capacity * (r + 1) / W;
+            G.index[r]->init_row_range(capacity, lo, hi);
+            gr->cfg = cfg;
+            gr->dist_mode = distance_mode(cfg.metric_kind, cfg.scalar_kind);
+            gr->row_bytes = G.index[r]->row_bytes_, gr->vec_bytes = G.index[r]->vec_bytes_;
+            gr->flags = search_view_flags();
+            if (cfg.M0 > 256)
+                throw CudaError("group: connectivity above 128 is not supported");
+            gr->borrowed = true, gr->capacity = capacity, gr->cap_lo = lo, gr->cap_hi = hi;
+            gr->attach(*G.index[r], *G.index[0]);
+            gr->allocate(max_batch, max_results, /*graph=*/false); // mailboxes and owner bitmaps sized for `capacity` rows
+        }
+        std::vector<PtrBlob> slabs(W);
+        for (size_t r = 0; r < W; ++r)
+            slabs[r] = G.ranks[r]->export_ptr(G.ranks[r]->slab);
+        for (size_t r = 0; r < W; ++r)
+            G.ranks[r]->map_peers(slabs.data());
+    } catch (...) {
+        for (GroupRank* r : G.ranks) {
+            r->release();
+            r->borrowed = false, r->capacity = 0;
+            r->d_rows = nullptr, r->d_adj0 = r->d_upper_ref = r->d_upper_adj = nullptr, r->d_keys = nullptr;
+        }
+        G.drop_index();
+        throw;
+    }
+    G.root = 0;
+    G.distributed = true;
+}
+
+// Host rows [0, n) (input kind f32 or b1, `stride` apart) -> rows [first, first + n) of the group's index: each row goes only to
+// the rank whose range holds it, cast to the storage kind there.  Rows travel through a bounded pinned block (two halves, as in
+// upload_file_rows) and a device block of the same size.
+static void upload_input_rows(Group& G, const uint8_t* vectors, size_t n, size_t stride, int kind, size_t first) {
+    const Index& root = *G.index[0];
+    const size_t in_bytes = scalar_row_bytes(kind, root.cfg_.dims), row_bytes = root.row_bytes_;
+    for (size_t r = 0; r < G.index.size(); ++r) {
+        Index& x = *G.index[r];
+        const size_t a = std::max(first, x.row_lo_), b = std::min(first + n, x.row_hi_);
+        if (a >= b)
+            continue;
+        LB_CUDA(cudaSetDevice(G.ranks[r]->device));
+        struct Staging {
+            uint8_t* pinned = nullptr;
+            void* raw = nullptr;
+            cudaStream_t stream = nullptr;
+            cudaEvent_t done[2] = {nullptr, nullptr};
+            ~Staging() {
+                if (stream)
+                    cudaStreamSynchronize(stream), cudaStreamDestroy(stream);
+                for (cudaEvent_t e : done)
+                    if (e)
+                        cudaEventDestroy(e);
+                cudaFreeHost(pinned), cudaFree(raw);
+            }
+        } st;
+        const size_t block = std::max<size_t>(1, std::min(b - a, ((size_t)16 << 20) / in_bytes)); // rows per half (<= 16 MB)
+        LB_CUDA(cudaMallocHost(&st.pinned, 2 * block * in_bytes));
+        LB_CUDA(cudaMalloc(&st.raw, 2 * block * in_bytes));
+        LB_CUDA(cudaStreamCreateWithFlags(&st.stream, cudaStreamNonBlocking));
+        LB_CUDA(cudaEventCreateWithFlags(&st.done[0], cudaEventDisableTiming));
+        LB_CUDA(cudaEventCreateWithFlags(&st.done[1], cudaEventDisableTiming));
+        bool used[2] = {false, false};
+        int h = 0;
+        for (size_t b0 = a; b0 < b; b0 += block, h ^= 1) {
+            const size_t cnt = std::min(block, b - b0);
+            uint8_t* stage = st.pinned + (size_t)h * block * in_bytes;
+            uint8_t* raw = (uint8_t*)st.raw + (size_t)h * block * in_bytes;
+            if (used[h])
+                LB_CUDA(cudaEventSynchronize(st.done[h]));
+            for (size_t i = 0; i < cnt; ++i)
+                memcpy(stage + i * in_bytes, vectors + (b0 - first + i) * stride, in_bytes);
+            LB_CUDA(cudaMemcpyAsync(raw, stage, cnt * in_bytes, cudaMemcpyHostToDevice, st.stream));
+            launch_cast_rows(raw, in_bytes, kind, x.d_vectors_ + (b0 - x.row_lo_) * row_bytes, row_bytes, root.cfg_.scalar_kind,
+                             root.cfg_.dims, cnt, st.stream);
+            LB_CUDA(cudaEventRecord(st.done[h], st.stream));
+            used[h] = true;
+        }
+        LB_CUDA(cudaStreamSynchronize(st.stream));
+    }
+}
+
+void group_index_add(Group& G, const uint64_t* keys, const void* vectors, size_t n, size_t stride, int kind) {
+    DeviceGuard dg;
+    std::lock_guard<std::mutex> lk(G.mu);
+    require_own_index(G);
+    Index& root = *G.index[0];
+    if (!(kind == SK_F32 || (kind == SK_B1 && root.cfg_.scalar_kind == SK_B1)))
+        throw CudaError("vectors must be passed as f32, or as packed bits (b1) for a b1 index");
+    if (!n)
+        return;
+    if (!keys || !vectors)
+        throw CudaError("null keys or vectors");
+    for (size_t i = 0; i < n; ++i)
+        if (keys[i] == ~0ull)
+            throw CudaError("key UINT64_MAX is reserved (free key)");
+    const size_t used = root.n_ + root.pending_n_;
+    if (used + n > root.capacity_)
+        throw CudaError("group index: " + std::to_string(n) + " more rows would pass the capacity of " + std::to_string(root.capacity_) +
+                        " rows fixed by lb200_group_index_init (" + std::to_string(used) + " held); nothing was added");
+    upload_input_rows(G, (const uint8_t*)vectors, n, stride, kind, used);
+    root.h_keys_.insert(root.h_keys_.end(), keys, keys + n);
+    root.pending_n_ += n;
+}
+
+// Inserts every pending row with all ranks, then points the search at the new graph.  Caller holds G.mu.
+static void group_index_build_locked(Group& G) {
+    Index& root = *G.index[0];
+    if (!root.pending_n_)
+        return;
+    std::vector<BuildReplica> shards = index_shards(G);
+    auto settle = [&] { // every rank's view of the graph state (the build updates the root's), scratch freed, search re-attached
+        for (size_t r = 0; r < shards.size(); ++r) {
+            Index& x = *shards[r].idx;
+            cudaSetDevice(shards[r].device);
+            x.n_ = root.n_, x.max_level_ = root.max_level_, x.entry_ = root.entry_, x.upper_lists_ = root.upper_lists_;
+            x.free_scratch();
+            G.ranks[r]->attach(x, root);
+        }
+    };
+    try {
+        LB_CUDA(cudaSetDevice(shards[0].device));
+        build_pending_group(root, shards, 0);
+    } catch (...) {
+        settle();
+        throw;
+    }
+    settle();
+}
+
+void group_index_build(Group& G) {
+    DeviceGuard dg;
+    std::lock_guard<std::mutex> lk(G.mu);
+    require_own_index(G);
+    group_index_build_locked(G);
+}
+
+void group_index_set_option(Group& G, const std::string& name, size_t value) {
+    std::lock_guard<std::mutex> lk(G.mu);
+    require_own_index(G);
+    Index& root = *G.index[0];
+    if (name == "build_batch")
+        root.build_batch_ = value;
+    else if (name == "build_ratio")
+        root.build_ratio_ = value ? value : 1;
+    else
+        throw CudaError("group index: unknown option (build_batch and build_ratio are available)");
+}
+
+size_t group_index_size(Group& G) {
+    std::lock_guard<std::mutex> lk(G.mu);
+    require_own_index(G);
+    return G.index[0]->size();
+}
+
+void group_index_build_stats(Group& G, size_t& vectors, uint64_t& distances, double& ms, size_t& value_bytes) {
+    std::lock_guard<std::mutex> lk(G.mu);
+    require_own_index(G);
+    const Index& root = *G.index[0];
+    vectors = root.last_build_n_, distances = root.last_build_dist_, ms = root.last_build_ms_, value_bytes = root.vec_bytes_;
+}
+
+size_t group_index_serialized_length(Group& G) {
+    DeviceGuard dg;
+    std::lock_guard<std::mutex> lk(G.mu);
+    require_own_index(G);
+    group_index_build_locked(G);
+    return G.index[0]->serialized_length_locked();
+}
+
+void group_index_save(Group& G, const std::function<void(size_t)>& length_ok, const std::function<void(const void*, size_t)>& write) {
+    DeviceGuard dg;
+    std::lock_guard<std::mutex> lk(G.mu);
+    require_own_index(G);
+    group_index_build_locked(G);
+    length_ok(G.index[0]->serialized_length_locked());
+    save_row_sharded(*G.index[0], index_shards(G), write);
+}
+
 // Message flags are (epoch mod 4096) << 20 | sequence number.  Before the 12-bit part wraps, every rank waits for its last
 // launch (which ends only when all ranks have finished theirs), all ranks meet, clear their mailboxes and meet again:
 // a word written 4096 launches ago can then never be mistaken for a fresh one.  Collective; costs two exchanges per 4095
@@ -1761,6 +2005,10 @@ void group_search_device(Group& G, const void* d_queries, size_t nq, size_t stri
         throw CudaError("group: device-buffer search is the multi-process entry point; use lb200_group_search_batch");
     if (!nq || !k)
         return;
+    if (!G.index.empty()) // the group's own index: pending rows first, as a one-GPU search does
+        group_index_build_locked(G);
+    if (G.ranks[0]->n == 0)
+        throw CudaError("group: the group's index is empty");
     GroupRank* r = G.ranks[0];
     const uint32_t L = beam_width(*r, k, ef);
     const uint32_t W = agree_W(G, L);
@@ -1777,6 +2025,20 @@ void group_search_host(Group& G, const void* queries, size_t nq, size_t stride, 
         throw CudaError("group: lb200_group_distribute has not been called");
     if (!nq || !k)
         return;
+    if (!G.index.empty()) { // the group's own index: pending rows first; an empty index finds nothing (index.hpp:2693)
+        group_index_build_locked(G);
+        if (G.index[0]->n_ == 0) {
+            for (size_t i = 0; i < nq * k; ++i) {
+                if (keys)
+                    keys[i] = ~0ull;
+                if (dists)
+                    dists[i] = INFINITY;
+            }
+            for (size_t i = 0; counts && i < nq; ++i)
+                counts[i] = 0;
+            return;
+        }
+    }
     const bool trace = getenv("LB200_GROUP_TRACE") != nullptr;
     auto now = [] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
     const double t0 = trace ? now() : 0;

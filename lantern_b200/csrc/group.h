@@ -3,6 +3,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <functional>
+#include <string>
+
 #include "../../include/lantern_b200.h"
 #include "engine.h"
 
@@ -69,5 +72,15 @@ void group_search_device(Group& G, const void* d_queries, size_t nq, size_t stri
 void group_search_host(Group& G, const void* queries, size_t nq, size_t stride, int kind, size_t k, size_t ef, uint64_t* keys,
                        float* dists, size_t* counts);
 void group_stats(Group& G, int which, GroupStats& out);
+// the group's own row-sharded index (single-process groups): rank r holds rows [capacity r / G, capacity (r+1) / G)
+void group_index_init(Group& G, const IndexConfig& cfg, size_t capacity, size_t max_batch, size_t max_results);
+void group_index_add(Group& G, const uint64_t* keys, const void* vectors, size_t n, size_t stride, int kind);
+void group_index_build(Group& G);
+void group_index_set_option(Group& G, const std::string& name, size_t value);
+size_t group_index_size(Group& G);
+void group_index_build_stats(Group& G, size_t& vectors, uint64_t& distances, double& ms, size_t& value_bytes);
+size_t group_index_serialized_length(Group& G);
+// length_ok(file length) may refuse (throw) before anything is written; write() then receives the whole file, in order
+void group_index_save(Group& G, const std::function<void(size_t)>& length_ok, const std::function<void(const void*, size_t)>& write);
 
 } // namespace lb200

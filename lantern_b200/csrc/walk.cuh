@@ -229,6 +229,8 @@ __device__ __forceinline__ float row_distance(const uint4 (&qreg)[NQ], const uin
 // state shared by every evaluator / walker
 struct WalkBase {
     static constexpr bool kScreen = false; // ScreenEval: the level-0 beam screens candidates before measuring them
+    static constexpr bool kRowTable = false; // RowEval<..., true>: rows addressed through a RowTable
+    static constexpr bool kTableWalker = false; // plain rows: a RowEval<..., true> twin exists (RowTableWalker)
     const GraphView& g; // the kernel's own (__grid_constant__) parameter: fields are read from the constant bank
     WalkSmem sm;
     uint32_t* vis;
@@ -259,8 +261,38 @@ struct WalkBase {
     }
 };
 
+// Where the rows of a replicated build live (build.cu): `count` contiguous ranges, range t = rows [hi[t-1], hi[t]) (hi[-1] = 0)
+// starting at base[t].  A full-replica group build passes one range, the rank's own copy; a row-sharded one passes every
+// rank's slice, peers' slices as peer-mapped pointers.  Range `own` is in this rank's memory and travels by bulk copy; the
+// PTX ISA does not say whether cp.async.bulk may read a peer-mapped address, so rows of the other ranges are read with
+// ordinary 16-byte loads (the same bytes land in the same ring slot, so no distance can differ).
+constexpr uint32_t kRowRangesMax = 8;
+struct RowTable {
+    uint32_t count, own;
+    uint32_t hi[kRowRangesMax];
+    const uint8_t* base[kRowRangesMax];
+    __device__ __forceinline__ const uint8_t* row(uint32_t id, uint32_t row_bytes, uint32_t& t) const {
+        uint32_t lo = 0;
+        t = 0;
+        while (t + 1 < count && id >= hi[t])
+            lo = hi[t++];
+        return base[t] + (size_t)(id - lo) * row_bytes;
+    }
+};
+
 // ---- evaluator for plain rows (f32 / f16 / i8 / b1): value in registers, rows through the bulk-copy ring --------
-template <int DM, int SK, int NQ> struct RowEval : WalkBase {
+// TABLE = rows are addressed through a RowTable (replicated build kernels only); otherwise at g.vectors + id * row_bytes.
+template <int DM, int SK, int NQ, bool TABLE = false> struct RowEval : WalkBase {
+    static constexpr bool kRowTable = TABLE;
+    static constexpr bool kTableWalker = true;
+    const RowTable* rows = nullptr; // TABLE: the kernel's own (__grid_constant__) table
+    __device__ __forceinline__ const uint8_t* row_addr(uint32_t id) const {
+        if constexpr (TABLE) {
+            uint32_t t;
+            return rows->row(id, g.row_bytes, t);
+        }
+        return g.vectors + (size_t)id * g.row_bytes;
+    }
     static __host__ __device__ WalkLayout layout(const GraphView& g, uint32_t R, uint32_t top_cap, uint32_t cand_cap) {
         return walk_layout(R, g.row_bytes, top_cap, cand_cap);
     }
@@ -292,13 +324,29 @@ template <int DM, int SK, int NQ> struct RowEval : WalkBase {
             a2 = n2;
     }
     // a stored node becomes the value (refine_: candidate vs accepted; reverse links: target vs its neighbours)
-    __device__ __forceinline__ void load_node(uint32_t id) { load_value(g.vectors + (size_t)id * g.row_bytes); }
+    __device__ __forceinline__ void load_node(uint32_t id) { load_value(row_addr(id)); }
     __device__ __forceinline__ void load_query(uint32_t, const uint8_t* row) { load_value(row); }
 
     __device__ __forceinline__ void issue(uint32_t slot, uint32_t id) {
         uint64_t* bar = &sm.full[slot];
-        mbar_arrive_expect_tx(bar, g.row_bytes);
-        bulk_g2s(sm.ring + (size_t)slot * g.row_bytes, g.vectors + (size_t)id * g.row_bytes, g.row_bytes, bar);
+        if constexpr (TABLE) {
+            uint32_t t;
+            const uint8_t* src = rows->row(id, g.row_bytes, t);
+            if (t != rows->own) { // a peer's row: this thread fills the slot, then arrives (release) without a transaction
+                const uint4* s = reinterpret_cast<const uint4*>(src);
+                uint4* d = reinterpret_cast<uint4*>(sm.ring + (size_t)slot * g.row_bytes);
+#pragma unroll 8
+                for (uint32_t c = 0; c < nchunks; ++c)
+                    d[c] = __ldg(s + c);
+                mbar_arrive(bar);
+                return;
+            }
+            mbar_arrive_expect_tx(bar, g.row_bytes);
+            bulk_g2s(sm.ring + (size_t)slot * g.row_bytes, src, g.row_bytes, bar);
+        } else {
+            mbar_arrive_expect_tx(bar, g.row_bytes);
+            bulk_g2s(sm.ring + (size_t)slot * g.row_bytes, g.vectors + (size_t)id * g.row_bytes, g.row_bytes, bar);
+        }
     }
 
     __device__ __forceinline__ float row_distance(const uint4* row) const { return lb200::row_distance<DM, SK, NQ>(qreg, row, nchunks, a2, lane); }
@@ -1009,6 +1057,14 @@ template <int DM, int SK, int NQ> using Walker = WalkerT<RowEval<DM, SK, NQ>>;
 template <int DM> using PqWalker = WalkerT<PqEval<DM>>;
 template <int DM, int NQ> using ScreenWalker = WalkerT<ScreenEval<DM, NQ>>;
 template <int DM, int NQ> using PScreenWalker = WalkerT<PScreenEval<DM, NQ>>;
+// the row-sharded build kernels' walker: plain-row walkers read through a RowTable; PQ walkers have none (a group index
+// cannot hold PQ codes)
+template <class W> struct RowTableWalker {
+    using type = W;
+};
+template <int DM, int SK, int NQ> struct RowTableWalker<WalkerT<RowEval<DM, SK, NQ>>> {
+    using type = WalkerT<RowEval<DM, SK, NQ, true>>;
+};
 
 // ---- (DM, SK, NQ) dispatch shared by the launchers ----------------------------------------------------
 // PQ indexes: fn(walker type tag) with PqWalker<DM>
