@@ -318,13 +318,15 @@ LB200_EXPORT void lb200_merge_shards_device(lb200_key_t const* d_keys, lb200_dis
  *                             (every rank passes `bytes_per_rank` bytes, everybody receives world * bytes_per_rank, rank
  *                             order); it is used at creation/distribution time only, never on the search path;
  *   lb200_group_create_local  one process driving n devices (what a Lantern indexing/search server would do).
- * and three ways to give it its graph (once per group):
+ * and four ways to give it its graph (once per group):
  *   lb200_group_distribute    the root rank passes a built (or loaded) index that lives on ITS device; every rank copies its
  *                             row range and the graph from it over NVLink.  The index must fit on one GPU.
  *   lb200_group_load[_buffer] every rank reads its row range and the graph straight from an index file; no GPU ever holds
  *                             all rows, so the group can serve an index larger than one GPU.
  *   lb200_group_index_init    the group gets an empty index of its own, fills it with lb200_group_index_add_batch and builds
  *                             it with all ranks (lb200_group_index_build); no GPU ever holds all rows here either.
+ *   lb200_group_index_load    the same index of its own, opened from an index file; it takes more rows, and
+ *                             lb200_group_index_reserve grows either kind past its capacity.
  * lb200_group_search_batch*: collective; only the root's queries are read (other ranks may pass NULL); EVERY rank receives
  * the full result (the final all-gather is fused into the kernel's epilogue: owners store their top-k into every rank). */
 typedef void* lb200_group_t;
@@ -383,17 +385,41 @@ LB200_EXPORT void lb200_group_rank_info(lb200_group_t, int local_rank, lb200_gro
 LB200_EXPORT void lb200_group_build(lb200_group_t, lb200_index_t root_index, int root, lb200_error_t* error);
 /* ---- the group's own index (single-process groups): built straight into the row-sharded layout, then searched and saved ----
  * lb200_group_index_init: the group gets an empty index with `options` (as lb200_init reads them) and room for `capacity`
- * rows.  Rank r holds rows [capacity r / G, capacity (r+1) / G) for the life of the group; lists and keys of all `capacity`
+ * rows.  Rank r holds rows [capacity r / G, capacity (r+1) / G) until lb200_group_index_reserve changes the capacity; lists and
+ * keys of all `capacity`
  * rows are kept on every rank.  max_batch / max_results: as in lb200_group_distribute.  PQ options are refused (a group
  * cannot hold PQ codes), and so are multi-process groups.  A group takes one lb200_group_distribute, lb200_group_load or
- * lb200_group_index_init, never two.  lb200_group_search_batch* and lb200_group_rank_info then work on this index; rank_info
+ * lb200_group_index_init (or lb200_group_index_load), never two.  lb200_group_search_batch* and lb200_group_rank_info then work
+ * on this index; rank_info
  * reports each rank's capacity range and bytes_rows for that range.  Pending rows are built by the next save or search, as
  * with a one-GPU index. */
 LB200_EXPORT void lb200_group_index_init(lb200_group_t, lb200_init_options_t const* options, size_t capacity, size_t max_batch,
                                          size_t max_results, lb200_error_t* error);
+/* lb200_group_index_load_buffer: the same kind of index as lb200_group_index_init gives, holding the contents of a
+ * usearch/lantern index file (written by this library or by usearch).  `options` is read as lb200_init reads it and is checked
+ * against the file exactly as lb200_load checks an index (metric, scalar kind, dimensions, connectivity; same messages);
+ * expansion_add and expansion_search come from `options`.  capacity 0 means the file's node count n; a capacity below n, or of
+ * 2^31 - 1 or more, is refused (an empty file needs a capacity of at least 1).  Rank r receives only the rows of [capacity r /
+ * G, capacity (r+1) / G), straight from `buffer` through a bounded pinned block; every rank receives the lists and keys.  The
+ * whole file is validated before any rank allocates: after a refusal the group can still take a correct load or an
+ * lb200_group_index_init.  The index then holds what lb200_load_buffer gives a one-GPU index (graph, keys, level generator), so
+ * the same adds and builds give the same file.  Refusals as in lb200_group_index_init (PQ, multi-process groups, a group that
+ * already holds a graph). */
+LB200_EXPORT void lb200_group_index_load_buffer(lb200_group_t, lb200_init_options_t const* options, void const* buffer,
+                                                size_t length, size_t capacity, size_t max_batch, size_t max_results,
+                                                lb200_error_t* error);
+/* the same from a file, mapped read-only (mmap): no host buffer and no GPU ever holds all rows */
+LB200_EXPORT void lb200_group_index_load(lb200_group_t, lb200_init_options_t const* options, char const* path,
+                                         size_t capacity, size_t max_batch, size_t max_results, lb200_error_t* error);
+/* As lb200_reserve: room for `capacity` rows; nothing happens at or below the current capacity.  Rank r's range becomes
+ * [capacity r / G, capacity (r+1) / G) and every row added so far, built or pending, moves to the rank whose new range holds
+ * it (device-to-device copies).  While the call runs, a rank holds its old and new rows and two copies of its level-0 lists,
+ * upper references and keys.  Every new array is allocated before any row moves: if one does not fit, the call fails naming
+ * the rank, device and what did not fit (rows, graph, scratch), and the index is left exactly as it was. */
+LB200_EXPORT void lb200_group_index_reserve(lb200_group_t, size_t capacity, lb200_error_t* error);
 /* Host rows, f32 or packed b1, with the input and key checks of lb200_add_batch.  Row i of the index goes only to the rank whose
  * range holds it, cast to the storage kind there, through a bounded pinned block.  Adding past `capacity` is refused and adds
- * nothing. */
+ * nothing (lb200_group_index_reserve raises it). */
 LB200_EXPORT void lb200_group_index_add_batch(lb200_group_t, lb200_key_t const* keys, void const* vectors, size_t n, size_t stride,
                                               lb200_scalar_kind_t kind, lb200_error_t* error);
 /* "build_batch" and "build_ratio", as lb200_set_option; the default batch cap is the one-GPU default times the ranks. */

@@ -163,6 +163,10 @@ SIGNATURES = {
     "lb200_group_rank_info": (None, [C.c_void_p, C.c_int, C.POINTER(GroupRankInfo), ERRP]),
     "lb200_group_build": (None, [C.c_void_p, C.c_void_p, C.c_int, ERRP]),
     "lb200_group_index_init": (None, [C.c_void_p, C.POINTER(InitOptions), C.c_size_t, C.c_size_t, C.c_size_t, ERRP]),
+    "lb200_group_index_load_buffer": (None, [C.c_void_p, C.POINTER(InitOptions), C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t,
+                                             C.c_size_t, ERRP]),
+    "lb200_group_index_load": (None, [C.c_void_p, C.POINTER(InitOptions), C.c_char_p, C.c_size_t, C.c_size_t, C.c_size_t, ERRP]),
+    "lb200_group_index_reserve": (None, [C.c_void_p, C.c_size_t, ERRP]),
     "lb200_group_index_add_batch": (None, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, ERRP]),
     "lb200_group_index_set_option": (None, [C.c_void_p, C.c_char_p, C.c_size_t, ERRP]),
     "lb200_group_index_build": (None, [C.c_void_p, ERRP]),
@@ -365,6 +369,7 @@ class Group:
                                     (concatenation of every rank's `send`, rank order), used for bootstrap only
     then once: distribute(index) (an index on the root's GPU) or load(path) / load_buffer(bytes) (each rank reads its rows)
                or index_init(capacity, ...) (an index of the group's own: index_add_batch, index_build, index_save)
+               or index_load(path, capacity, ...) / index_load_buffer (the same, opened from a file); index_reserve grows it
     """
 
     def __init__(self, handle, world, keep=None):
@@ -453,6 +458,26 @@ class Group:
         """An empty index of the group's own with room for `capacity` rows; rank r holds rows [capacity r / G, capacity (r+1) / G)."""
         o = init_options(dim, metric, quant, M, efc, ef, pq)
         self._call("lb200_group_index_init", C.byref(o), capacity, max_batch, max_results)
+
+    def index_load_buffer(self, buf, capacity, dim, metric="l2sq", quant="f32", M=16, efc=128, ef=64, pq=False, max_batch=8192,
+                          max_results=0):
+        """An index of the group's own whose contents come from index file bytes, with room for `capacity` rows (0 = the
+        file's rows); rank r receives only the rows of [capacity r / G, capacity (r+1) / G).  The options are checked against
+        the file as Index.load_buffer checks them."""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        o = init_options(dim, metric, quant, M, efc, ef, pq)
+        self._call("lb200_group_index_load_buffer", C.byref(o), _ptr(buf), len(buf), capacity, max_batch, max_results)
+
+    def index_load(self, path, capacity, dim, metric="l2sq", quant="f32", M=16, efc=128, ef=64, pq=False, max_batch=8192,
+                   max_results=0):
+        """index_load_buffer from a file, mapped read-only by the engine."""
+        o = init_options(dim, metric, quant, M, efc, ef, pq)
+        self._call("lb200_group_index_load", C.byref(o), path.encode(), capacity, max_batch, max_results)
+
+    def index_reserve(self, capacity):
+        """Room for `capacity` rows (nothing happens at or below the current capacity): the ranges become
+        [capacity r / G, capacity (r+1) / G) and the rows move to the ranks that now hold them."""
+        self._call("lb200_group_index_reserve", capacity)
 
     def index_add_batch(self, keys, vecs):
         vecs = np.ascontiguousarray(vecs)

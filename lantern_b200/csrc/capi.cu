@@ -918,6 +918,31 @@ LB200_EXPORT void lb200_group_index_init(lb200_group_t h, lb200_init_options_t c
         group_index_init(G, cfg, capacity, group_max_batch(max_batch), group_max_results(max_batch, max_results));
     });
 }
+LB200_EXPORT void lb200_group_index_load_buffer(lb200_group_t h, lb200_init_options_t const* options, void const* buffer,
+                                                size_t length, size_t capacity, size_t max_batch, size_t max_results,
+                                                lb200_error_t* error) {
+    guarded(error, [&] {
+        Group& G = *as_group(h);
+        const IndexConfig cfg = group_load_config(options);
+        if (!buffer && length)
+            throw CudaError("null buffer");
+        group_index_load(G, cfg, buffer, length, capacity, group_max_batch(max_batch), group_max_results(max_batch, max_results));
+    });
+}
+LB200_EXPORT void lb200_group_index_load(lb200_group_t h, lb200_init_options_t const* options, char const* path, size_t capacity,
+                                         size_t max_batch, size_t max_results, lb200_error_t* error) {
+    guarded(error, [&] {
+        Group& G = *as_group(h);
+        const IndexConfig cfg = group_load_config(options);
+        if (!path)
+            throw CudaError("null path");
+        MappedFile f(path);
+        group_index_load(G, cfg, f.data(), f.length, capacity, group_max_batch(max_batch), group_max_results(max_batch, max_results));
+    });
+}
+LB200_EXPORT void lb200_group_index_reserve(lb200_group_t h, size_t capacity, lb200_error_t* error) {
+    guarded(error, [&] { group_index_reserve(*as_group(h), capacity); });
+}
 LB200_EXPORT void lb200_group_index_add_batch(lb200_group_t h, lb200_key_t const* keys, void const* vectors, size_t n, size_t stride,
                                               lb200_scalar_kind_t kind, lb200_error_t* error) {
     guarded(error, [&] { group_index_add(*as_group(h), keys, vectors, n, stride, kind); });

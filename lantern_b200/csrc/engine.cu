@@ -130,6 +130,16 @@ void Index::init_row_range(size_t capacity, size_t lo, size_t hi) {
     sharded_ = true, row_lo_ = lo, row_hi_ = hi;
 }
 
+void Index::replace_row_range(size_t capacity, size_t lo, size_t hi, uint8_t* vectors, uint32_t* adj0, uint32_t* upper_ref,
+                              uint64_t* keys) {
+    if (!sharded_ || lo > hi || hi > capacity || capacity < n_ + pending_n_)
+        throw CudaError("index: a new row range needs a row-sharded index, lo <= hi <= capacity and room for its rows");
+    cudaFree(d_vectors_), cudaFree(d_adj0_), cudaFree(d_upper_ref_), cudaFree(d_keys_);
+    d_vectors_ = vectors, d_adj0_ = adj0, d_upper_ref_ = upper_ref, d_keys_ = keys;
+    free_scratch(); // the build's visited bitmaps are sized for the capacity
+    capacity_ = capacity, row_lo_ = lo, row_hi_ = hi;
+}
+
 void Index::free_scratch() {
     cudaFree(scratch_.visited), cudaFree(scratch_.touched);
     scratch_.visited = nullptr, scratch_.touched = nullptr;

@@ -177,6 +177,14 @@ class Index {
     // one rank's part of a group's own index (group.cu): d_vectors_ holds rows [lo, hi) only (row i at (i - lo) * row_bytes_);
     // lists, levels and keys are sized for all `capacity` rows.  No search-screen companion.  Called once, on an empty index.
     void init_row_range(size_t capacity, size_t lo, size_t hi);
+    // the same index at a new capacity and row range, contents kept: the caller has copied rows [lo, min(hi, size)) into
+    // `vectors` and the lists, upper references and keys of all rows into arrays sized for `capacity` (0xFF beyond them);
+    // the old arrays and the build scratch are freed.  Nothing here allocates or throws once the arguments pass.
+    void replace_row_range(size_t capacity, size_t lo, size_t hi, uint8_t* vectors, uint32_t* adj0, uint32_t* upper_ref, uint64_t* keys);
+    // the graph state of a parsed file (format.cu): lists, upper references and keys on the device (0xFF beyond them), then
+    // n, entry, top level and upper-list count; `host_mirrors`: the levels and keys on the host too, moved out of `f`.  The
+    // rows are the caller's, and so is a capacity of at least f.n.  The level generator is not touched.
+    void commit_file_graph(ParsedIndexFile& f, bool host_mirrors);
     void free_scratch(); // the visited bitmaps and touched lists (they grow with capacity x resident CTAs)
 
     IndexConfig cfg_;

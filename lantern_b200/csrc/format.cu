@@ -281,11 +281,7 @@ void Index::load_buffer(const void* buffer, size_t length) {
     std::lock_guard<std::mutex> g(mu_);
     ParsedIndexFile f;
     parse_index_file(cfg_, vec_bytes_, stored_bytes_, buffer, length, f);
-    const size_t n = f.n, M = cfg_.M, M0 = cfg_.M0;
-    const std::vector<uint32_t>& adj0 = f.adj0;
-    const std::vector<uint32_t>& upper_ref = f.upper_ref;
-    const std::vector<uint32_t>& upper_adj = f.upper_adj;
-    std::vector<uint64_t>& keys = f.keys;
+    const size_t n = f.n;
     std::vector<uint8_t> rows(n * row_bytes_, 0);
     for (size_t i = 0; i < n; ++i)
         memcpy(rows.data() + i * row_bytes_, (const uint8_t*)buffer + f.row_off[i], stored_bytes_);
@@ -305,29 +301,41 @@ void Index::load_buffer(const void* buffer, size_t length) {
     n_ = 0, pending_n_ = 0;
     ensure_capacity(n ? n : 1);
     reset_screen(); // the screen is chosen again from the loaded rows
+    if (n) {
+        LB_CUDA(cudaMemcpy(d_vectors_, rows.data(), rows.size(), cudaMemcpyHostToDevice));
+        encode_screen(0, n);
+    }
+    commit_file_graph(f, true);
+    decide_screen();
+}
+
+// load_buffer's commit of the graph, shared with a group index's load (group.cu)
+void Index::commit_file_graph(ParsedIndexFile& f, bool host_mirrors) {
+    const size_t n = f.n, M = cfg_.M, M0 = cfg_.M0;
     upper_lists_ = 0;
-    alloc_upper(upper_adj.size() / M + 1);
+    alloc_upper(f.upper_adj.size() / M + 1);
     // everything beyond the loaded nodes / lists must read as empty (0xFF): a later insert with level > max_level exposes
     // its still-unwritten upper lists to greedy() before build_insert_kernel has filled them
     LB_CUDA(cudaMemset(d_adj0_, 0xFF, capacity_ * M0 * 4));
     LB_CUDA(cudaMemset(d_upper_ref_, 0xFF, capacity_ * 4));
     LB_CUDA(cudaMemset(d_upper_adj_, 0xFF, upper_lists_cap_ * M * 4));
     if (n) {
-        LB_CUDA(cudaMemcpy(d_vectors_, rows.data(), rows.size(), cudaMemcpyHostToDevice));
-        encode_screen(0, n);
-        LB_CUDA(cudaMemcpy(d_adj0_, adj0.data(), adj0.size() * 4, cudaMemcpyHostToDevice));
-        LB_CUDA(cudaMemcpy(d_upper_ref_, upper_ref.data(), upper_ref.size() * 4, cudaMemcpyHostToDevice));
-        if (!upper_adj.empty())
-            LB_CUDA(cudaMemcpy(d_upper_adj_, upper_adj.data(), upper_adj.size() * 4, cudaMemcpyHostToDevice));
-        LB_CUDA(cudaMemcpy(d_keys_, keys.data(), keys.size() * 8, cudaMemcpyHostToDevice));
+        LB_CUDA(cudaMemcpy(d_adj0_, f.adj0.data(), f.adj0.size() * 4, cudaMemcpyHostToDevice));
+        LB_CUDA(cudaMemcpy(d_upper_ref_, f.upper_ref.data(), f.upper_ref.size() * 4, cudaMemcpyHostToDevice));
+        if (!f.upper_adj.empty())
+            LB_CUDA(cudaMemcpy(d_upper_adj_, f.upper_adj.data(), f.upper_adj.size() * 4, cudaMemcpyHostToDevice));
+        LB_CUDA(cudaMemcpy(d_keys_, f.keys.data(), f.keys.size() * 8, cudaMemcpyHostToDevice));
     }
-    upper_lists_ = upper_adj.size() / M;
-    h_levels_ = std::move(f.levels);
-    h_keys_ = std::move(keys);
+    upper_lists_ = f.upper_adj.size() / M;
+    if (host_mirrors) {
+        h_levels_ = std::move(f.levels);
+        h_keys_ = std::move(f.keys);
+    } else {
+        h_levels_.clear(), h_keys_.clear();
+    }
     n_ = n;
     max_level_ = f.max_level;
     entry_ = f.entry;
-    decide_screen();
 }
 
 } // namespace lb200

@@ -1754,7 +1754,7 @@ void group_build(Group& G, Index* root_index, int root) {
 
 static void require_own_index(Group& G) {
     if (G.index.empty())
-        throw CudaError("group index: lb200_group_index_init has not been called on this group");
+        throw CudaError("group index: lb200_group_index_init (or lb200_group_index_load) has not been called on this group");
 }
 
 static std::vector<BuildReplica> index_shards(Group& G) {
@@ -1764,9 +1764,8 @@ static std::vector<BuildReplica> index_shards(Group& G) {
     return s;
 }
 
-void group_index_init(Group& G, const IndexConfig& cfg, size_t capacity, size_t max_batch, size_t max_results) {
-    DeviceGuard dg;
-    std::lock_guard<std::mutex> lk(G.mu);
+// the refusals every way of giving a group an index of its own shares; caller holds G.mu
+static void check_own_index_formation(Group& G, const IndexConfig& cfg) {
     if (G.ranks.size() != (size_t)G.world)
         throw CudaError("group index: a multi-process group cannot hold an index of its own; create the group with "
                         "lb200_group_create_local");
@@ -1775,16 +1774,33 @@ void group_index_init(Group& G, const IndexConfig& cfg, size_t capacity, size_t 
                         "lb200_group_index_init per group)");
     if (cfg.pq)
         throw CudaError("group index: pq indexes are not supported");
-    if (capacity == 0 || capacity >= 0x7FFFFFFFull)
-        throw CudaError("group index: capacity must be in [1, 2^31 - 1)");
+}
+
+// An index of `capacity` rows of the group's own: empty, or holding a parsed file `f` (whose node i's bytes are at
+// file + f->row_off[i]).  Rank r's index gets the rows of [capacity r / G, capacity (r+1) / G) only -- copied from the file
+// bytes through upload_file_rows' bounded pinned block -- and the lists, upper lists and keys of the whole graph; rank 0 also
+// keeps the levels and keys on the host.  On a failure nothing stays allocated.  Caller holds G.mu.
+static void form_own_index(Group& G, const IndexConfig& cfg, size_t capacity, size_t max_batch, size_t max_results,
+                           ParsedIndexFile* f, const uint8_t* file) {
     const size_t W = (size_t)G.world;
     try {
         for (size_t r = 0; r < W; ++r) {
+            LB_CUDA(cudaSetDevice(G.ranks[r]->device));
+            G.index.emplace_back(new Index(cfg, nullptr));
+            G.index[r]->init_row_range(capacity, capacity * r / W, capacity * (r + 1) / W);
+        }
+        for (size_t r = W; f && r-- > 0;) { // (rank 0 last: its commit moves the host levels and keys out of `f`)
+            Index& x = *G.index[r];
+            LB_CUDA(cudaSetDevice(G.ranks[r]->device));
+            x.commit_file_graph(*f, r == 0);
+            LB_CUDA(cudaDeviceSynchronize()); // (init_row_range's zero fill ran on the legacy stream; the upload has its own)
+            upload_file_rows(file, f->row_off, x.stored_bytes_, x.row_lo_, std::min(x.row_hi_, f->n), x.d_vectors_, x.row_bytes_);
+            LB_CUDA(cudaDeviceSynchronize());
+        }
+        for (size_t r = 0; r < W; ++r) {
             GroupRank* gr = G.ranks[r];
             LB_CUDA(cudaSetDevice(gr->device));
-            G.index.emplace_back(new Index(cfg, nullptr));
-            const size_t lo = capacity * r / W, hi = capacity * (r + 1) / W;
-            G.index[r]->init_row_range(capacity, lo, hi);
+            const size_t lo = G.index[r]->row_lo_, hi = G.index[r]->row_hi_;
             gr->cfg = cfg;
             gr->dist_mode = distance_mode(cfg.metric_kind, cfg.scalar_kind);
             gr->row_bytes = G.index[r]->row_bytes_, gr->vec_bytes = G.index[r]->vec_bytes_;
@@ -1811,6 +1827,137 @@ void group_index_init(Group& G, const IndexConfig& cfg, size_t capacity, size_t 
     }
     G.root = 0;
     G.distributed = true;
+}
+
+void group_index_init(Group& G, const IndexConfig& cfg, size_t capacity, size_t max_batch, size_t max_results) {
+    DeviceGuard dg;
+    std::lock_guard<std::mutex> lk(G.mu);
+    check_own_index_formation(G, cfg);
+    if (capacity == 0 || capacity >= 0x7FFFFFFFull)
+        throw CudaError("group index: capacity must be in [1, 2^31 - 1)");
+    form_own_index(G, cfg, capacity, max_batch, max_results, nullptr, nullptr);
+}
+
+void group_index_load(Group& G, const IndexConfig& cfg, const void* buffer, size_t length, size_t capacity, size_t max_batch,
+                      size_t max_results) {
+    DeviceGuard dg;
+    std::lock_guard<std::mutex> lk(G.mu);
+    check_own_index_formation(G, cfg);
+    // the whole file is parsed and checked, as Index::load_buffer checks it, before any rank allocates
+    const size_t vec_bytes = scalar_row_bytes(cfg.scalar_kind, cfg.dims);
+    ParsedIndexFile f;
+    parse_index_file(cfg, vec_bytes, vec_bytes, buffer, length, f);
+    if (capacity == 0)
+        capacity = f.n;
+    if (capacity < std::max<size_t>(f.n, 1) || capacity >= 0x7FFFFFFFull)
+        throw CudaError("group index: capacity must be in [max(1, rows in the file), 2^31 - 1); the file holds " +
+                        std::to_string(f.n) + " rows");
+    form_own_index(G, cfg, capacity, max_batch, max_results, &f, (const uint8_t*)buffer);
+}
+
+// Raises the capacity of the group's own index to `capacity`: rank r's range becomes [capacity r / G, capacity (r+1) / G)
+// and rows [0, n + pending) move into the new row arrays of the ranks that now hold them, one copy-engine copy per (old rank,
+// new rank) overlap.  Every new array of every rank is allocated before any row moves; on a failure they are all freed and
+// the index is left as it was.  While the call runs a rank holds its old and new rows and two copies of its level-0 lists,
+// upper references and keys.  The mailbox slab does not depend on the capacity (slab_layout takes M0), so the peers' mappings
+// stay; the owner bitmaps (words_per_slot) do, and are replaced.
+void group_index_reserve(Group& G, size_t capacity) {
+    DeviceGuard dg;
+    std::lock_guard<std::mutex> lk(G.mu);
+    require_own_index(G);
+    Index& root = *G.index[0];
+    if (capacity <= root.capacity_)
+        return; // as lb200_reserve
+    if (capacity >= 0x7FFFFFFFull)
+        throw CudaError("group index: capacity must be in [1, 2^31 - 1)");
+    const size_t W = G.index.size(), n = root.n_, used = root.n_ + root.pending_n_, M0 = root.cfg_.M0, rb = root.row_bytes_;
+    struct Fresh { // one rank's new arrays until they are handed over
+        int device = 0;
+        uint8_t* rows = nullptr;
+        uint32_t *adj0 = nullptr, *upper_ref = nullptr, *vis = nullptr;
+        uint64_t* keys = nullptr;
+        cudaStream_t stream = nullptr;
+        size_t lo = 0, hi = 0, words_per_slot = 0;
+    };
+    struct FreshAll {
+        std::vector<Fresh> f;
+        bool handed_over = false;
+        ~FreshAll() {
+            for (Fresh& x : f) {
+                cudaSetDevice(x.device);
+                if (x.stream)
+                    cudaStreamSynchronize(x.stream), cudaStreamDestroy(x.stream);
+                if (!handed_over)
+                    cudaFree(x.rows), cudaFree(x.adj0), cudaFree(x.upper_ref), cudaFree(x.keys), cudaFree(x.vis);
+            }
+        }
+    } fresh;
+    fresh.f.resize(W);
+    // every allocation first, named by rank, device and what it holds
+    for (size_t r = 0; r < W; ++r) {
+        GroupRank& gr = *G.ranks[r];
+        Fresh& x = fresh.f[r];
+        x.device = gr.device;
+        x.lo = capacity * r / W, x.hi = capacity * (r + 1) / W;
+        x.words_per_slot = round_up((capacity + 31) / 32, 32);
+        LB_CUDA(cudaSetDevice(gr.device));
+        gr.device_alloc(&x.rows, std::max<size_t>((x.hi - x.lo) * rb, 16), "rows");
+        gr.device_alloc(&x.adj0, capacity * M0 * 4, "graph (lists, keys)");
+        gr.device_alloc(&x.upper_ref, capacity * 4, "graph (lists, keys)");
+        gr.device_alloc(&x.keys, capacity * 8, "graph (lists, keys)");
+        gr.device_alloc(&x.vis, (size_t)gr.Omax * x.words_per_slot * 4, "scratch (visited bitmaps)");
+        LB_CUDA(cudaStreamCreateWithFlags(&x.stream, cudaStreamNonBlocking));
+    }
+    for (size_t r = 0; r < W; ++r) { // (earlier work on the old arrays may still be queued on the legacy stream)
+        LB_CUDA(cudaSetDevice(fresh.f[r].device));
+        LB_CUDA(cudaDeviceSynchronize());
+    }
+    // the graph arrays grow as grow_device grows them (0xFF beyond the built nodes); rows beyond n + pending are zero, as
+    // init_row_range leaves them
+    for (size_t r = 0; r < W; ++r) {
+        Index& old = *G.index[r];
+        Fresh& x = fresh.f[r];
+        LB_CUDA(cudaSetDevice(x.device));
+        LB_CUDA(cudaMemsetAsync(x.rows, 0, std::max<size_t>((x.hi - x.lo) * rb, 16), x.stream));
+        LB_CUDA(cudaMemsetAsync(x.adj0, 0xFF, capacity * M0 * 4, x.stream));
+        LB_CUDA(cudaMemsetAsync(x.upper_ref, 0xFF, capacity * 4, x.stream));
+        LB_CUDA(cudaMemsetAsync(x.keys, 0xFF, capacity * 8, x.stream));
+        LB_CUDA(cudaMemsetAsync(x.vis, 0, (size_t)G.ranks[r]->Omax * x.words_per_slot * 4, x.stream));
+        if (n) {
+            LB_CUDA(cudaMemcpyAsync(x.adj0, old.d_adj0_, n * M0 * 4, cudaMemcpyDeviceToDevice, x.stream));
+            LB_CUDA(cudaMemcpyAsync(x.upper_ref, old.d_upper_ref_, n * 4, cudaMemcpyDeviceToDevice, x.stream));
+            LB_CUDA(cudaMemcpyAsync(x.keys, old.d_keys_, n * 8, cudaMemcpyDeviceToDevice, x.stream));
+        }
+    }
+    // rows [0, used): one peer copy per (old rank s, new rank t) overlap, on the receiving rank's stream (after its memset)
+    for (size_t t = 0; t < W; ++t) {
+        Fresh& x = fresh.f[t];
+        LB_CUDA(cudaSetDevice(x.device));
+        for (size_t s = 0; s < W; ++s) {
+            const Index& old = *G.index[s];
+            const size_t a = std::max(old.row_lo_, x.lo), b = std::min(std::min(old.row_hi_, x.hi), used);
+            if (a < b)
+                LB_CUDA(cudaMemcpyPeerAsync(x.rows + (a - x.lo) * rb, x.device, old.d_vectors_ + (a - old.row_lo_) * rb,
+                                            G.ranks[s]->device, (b - a) * rb, x.stream));
+        }
+    }
+    for (size_t r = 0; r < W; ++r) {
+        LB_CUDA(cudaSetDevice(fresh.f[r].device));
+        LB_CUDA(cudaStreamSynchronize(fresh.f[r].stream));
+    }
+    // hand over: nothing below allocates or throws
+    fresh.handed_over = true;
+    for (size_t r = 0; r < W; ++r) {
+        GroupRank& gr = *G.ranks[r];
+        Fresh& x = fresh.f[r];
+        cudaSetDevice(x.device);
+        G.index[r]->replace_row_range(capacity, x.lo, x.hi, x.rows, x.adj0, x.upper_ref, x.keys);
+        cudaFree(gr.d_vis);
+        gr.d_vis = x.vis, gr.words_per_slot = x.words_per_slot;
+        gr.capacity = capacity, gr.cap_lo = x.lo, gr.cap_hi = x.hi;
+    }
+    for (size_t r = 0; r < W; ++r)
+        G.ranks[r]->attach(*G.index[r], root);
 }
 
 // Host rows [0, n) (input kind f32 or b1, `stride` apart) -> rows [first, first + n) of the group's index: each row goes only to
@@ -1882,7 +2029,7 @@ void group_index_add(Group& G, const uint64_t* keys, const void* vectors, size_t
     const size_t used = root.n_ + root.pending_n_;
     if (used + n > root.capacity_)
         throw CudaError("group index: " + std::to_string(n) + " more rows would pass the capacity of " + std::to_string(root.capacity_) +
-                        " rows fixed by lb200_group_index_init (" + std::to_string(used) + " held); nothing was added");
+                        " rows (" + std::to_string(used) + " held; lb200_group_index_reserve raises it); nothing was added");
     upload_input_rows(G, (const uint8_t*)vectors, n, stride, kind, used);
     root.h_keys_.insert(root.h_keys_.end(), keys, keys + n);
     root.pending_n_ += n;

@@ -74,6 +74,12 @@ void group_search_host(Group& G, const void* queries, size_t nq, size_t stride, 
 void group_stats(Group& G, int which, GroupStats& out);
 // the group's own row-sharded index (single-process groups): rank r holds rows [capacity r / G, capacity (r+1) / G)
 void group_index_init(Group& G, const IndexConfig& cfg, size_t capacity, size_t max_batch, size_t max_results);
+// the same index holding the contents of an index file (capacity 0 = the file's rows); `cfg` is checked against the file as
+// Index::load_buffer checks it
+void group_index_load(Group& G, const IndexConfig& cfg, const void* buffer, size_t length, size_t capacity, size_t max_batch,
+                      size_t max_results);
+// raises the capacity (nothing happens at or below it): new ranges [capacity r / G, capacity (r+1) / G), rows moved between ranks
+void group_index_reserve(Group& G, size_t capacity);
 void group_index_add(Group& G, const uint64_t* keys, const void* vectors, size_t n, size_t stride, int kind);
 void group_index_build(Group& G);
 void group_index_set_option(Group& G, const std::string& name, size_t value);
