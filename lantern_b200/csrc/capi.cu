@@ -471,12 +471,19 @@ LB200_EXPORT uint64_t lb200_header_get_entry_slot(char* headerp) {
 }
 LB200_EXPORT void lb200_header_set_entry_slot(char* headerp, uint64_t entry_slot) { memcpy(headerp + 80 + 32, &entry_slot, 6); }
 
+// i8 distances come from int32 dot products (dp4a): exact up to 131071 dimensions, where 128^2 d still fits
+static void check_i8_dims(int scalar_kind, size_t dims) {
+    if (scalar_kind == SK_I8 && dims > 131071)
+        throw CudaError("i8 rows wider than 131071 dimensions are not supported");
+}
+
 LB200_EXPORT void lb200_distance_batch(void const* a, size_t a_stride, void const* b, size_t b_stride, size_t n,
                                        lb200_scalar_kind_t scalar_kind, size_t dimensions, lb200_metric_kind_t metric_kind,
                                        lb200_distance_t* out, lb200_error_t* error) {
     guarded(error, [&] {
         require_device();
         check_metric_scalar(metric_kind, scalar_kind);
+        check_i8_dims(scalar_kind, dimensions);
         if (!n)
             return;
         const size_t rb = round_up(scalar_row_bytes(scalar_kind, dimensions), 16);
@@ -505,6 +512,7 @@ LB200_EXPORT void lb200_exact_search_device(void const* d_dataset, size_t datase
     guarded(error, [&] {
         require_device();
         check_metric_scalar(metric_kind, scalar_kind);
+        check_i8_dims(scalar_kind, dimensions);
         cudaStream_t stream = (cudaStream_t)cuda_stream;
         const size_t bytes = scalar_row_bytes(scalar_kind, dimensions);
         const size_t rb = round_up(bytes, 16);
@@ -541,6 +549,7 @@ LB200_EXPORT void lb200_exact_search(void const* dataset, size_t dataset_size, s
     guarded(error, [&] {
         require_device();
         check_metric_scalar(metric_kind, scalar_kind);
+        check_i8_dims(scalar_kind, dimensions);
         if (!queries_size || !count)
             return;
         const size_t rb = round_up(scalar_row_bytes(scalar_kind, dimensions), 16);

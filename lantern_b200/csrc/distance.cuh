@@ -162,10 +162,12 @@ template <int DM, int SK> __device__ __forceinline__ float finish_distance(const
         return (float)warp_sum_u32(a.v[0] + a.v[1] + a.v[2] + a.v[3]);
     } else if constexpr (SK == SK_I8) {
         if constexpr (DM == DM_L2SQ) {
-            int qq = (int)warp_sum_u32((uint32_t)a.v[0]);
-            int rr = (int)warp_sum_u32((uint32_t)a.v[1]);
-            int qr = (int)warp_sum_u32((uint32_t)a.v[2]);
-            return (float)(qq + rr - 2 * qr);
+            // |q|^2 and |r|^2 are below 2^32 and q.r within int32 up to 131071 dimensions (the exhaustive search and the
+            // pair distances refuse wider i8 rows); their combination reaches 255^2 d and is formed in 64 bits
+            const uint32_t qq = warp_sum_u32((uint32_t)a.v[0]);
+            const uint32_t rr = warp_sum_u32((uint32_t)a.v[1]);
+            const int qr = (int)warp_sum_u32((uint32_t)a.v[2]);
+            return (float)((long long)qq + (long long)rr - 2ll * qr);
         } else {
             float ab = (float)(int)warp_sum_u32((uint32_t)a.v[0]);
             float b2 = (float)(int)warp_sum_u32((uint32_t)a.v[2]);

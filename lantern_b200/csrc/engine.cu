@@ -28,6 +28,13 @@ int device_sm_count() {
     return sms;
 }
 
+size_t device_smem_optin() {
+    int dev = 0, limit = 0;
+    LB_CUDA(cudaGetDevice(&dev));
+    LB_CUDA(cudaDeviceGetAttribute(&limit, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    return (size_t)limit;
+}
+
 void require_device() {
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);

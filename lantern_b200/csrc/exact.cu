@@ -12,6 +12,7 @@
 #include <stdlib.h>
 #include <math.h>
 
+#include <algorithm>
 #include <type_traits>
 
 #include "distance.cuh"
@@ -57,44 +58,58 @@ __device__ __forceinline__ void list_insert(float* ld, uint64_t* li, uint32_t& s
     size = last + 1;
 }
 
-// grid = (dataset blocks, query tiles).  Partial results: part_*[block][query][k].
-template <int DM, int SK>
+// grid = (dataset blocks, query tiles), the tiles counted from `tile0`.  Partial results: part_*[block][query][k].
+// QG: the kQT query rows are read from global memory (L1 / L2) instead of being staged in shared memory -- for rows so wide
+// that kQT of them and the top-k lists exceed the opt-in shared memory of a CTA.  A tile's missing queries (past nq) then
+// read the last query; their distances are computed and dropped.
+template <int DM, int SK, bool QG>
 __global__ void __launch_bounds__(kExWarps * 32) exact_block_kernel(const uint8_t* __restrict__ data, size_t n, size_t data_stride,
                                                                     const uint8_t* __restrict__ queries, uint32_t nq,
                                                                     size_t q_stride, uint32_t row_bytes, uint32_t k,
-                                                                    uint32_t rows_per_block, uint64_t* __restrict__ part_keys,
+                                                                    uint32_t rows_per_block, uint32_t tile0,
+                                                                    uint64_t* __restrict__ part_keys,
                                                                     float* __restrict__ part_dists,
                                                                     const uint8_t* __restrict__ qmask) {
     extern __shared__ __align__(16) uint8_t sm_raw[];
+    const uint32_t q0 = (tile0 + blockIdx.y) * kQT;
     if (qmask) { // second pass behind the tensor-core filter (exact_tc.cu): only the queries it could not certify
         bool any = false;
         for (uint32_t q = 0; q < kQT; ++q)
-            any |= blockIdx.y * kQT + q < nq && qmask[blockIdx.y * kQT + q];
+            any |= q0 + q < nq && qmask[q0 + q];
         if (!any)
             return;
     }
     const uint32_t nchunks = row_bytes / 16;
-    uint4* sq = reinterpret_cast<uint4*>(sm_raw);                                // [kQT][nchunks]
-    float* sdist = reinterpret_cast<float*>(sm_raw + (size_t)kQT * row_bytes);     // [kQT][kSub]
+    const size_t sq_bytes = QG ? 0 : (size_t)kQT * row_bytes;
+    uint4* sq = reinterpret_cast<uint4*>(sm_raw);                                // [kQT][nchunks] (not QG)
+    float* sdist = reinterpret_cast<float*>(sm_raw + sq_bytes);                    // [kQT][kSub]
     float* ld = sdist + kQT * kSub;                                               // [kQT][k]
     uint64_t* li = reinterpret_cast<uint64_t*>(ld + (((size_t)kQT * k + 1) & ~(size_t)1)); // [kQT][k]
     __shared__ float sa2[kQT];
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t q0 = blockIdx.y * kQT;
     const size_t row0 = (size_t)blockIdx.x * rows_per_block;
     const size_t row1 = min(n, row0 + rows_per_block);
+    // chunk c of query q0 + q
+    auto qchunk = [&](int q, uint32_t c) -> uint4 {
+        if constexpr (QG)
+            return __ldg(reinterpret_cast<const uint4*>(queries + (size_t)min(q0 + q, nq - 1) * q_stride) + c);
+        else
+            return sq[q * nchunks + c];
+    };
 
-    for (uint32_t i = threadIdx.x; i < kQT * nchunks; i += blockDim.x) {
-        uint32_t q = i / nchunks, c = i % nchunks;
-        sq[i] = (q0 + q < nq) ? __ldg(reinterpret_cast<const uint4*>(queries + (size_t)(q0 + q) * q_stride) + c)
-                              : make_uint4(0, 0, 0, 0);
+    if constexpr (!QG) {
+        for (uint32_t i = threadIdx.x; i < kQT * nchunks; i += blockDim.x) {
+            uint32_t q = i / nchunks, c = i % nchunks;
+            sq[i] = (q0 + q < nq) ? __ldg(reinterpret_cast<const uint4*>(queries + (size_t)(q0 + q) * q_stride) + c)
+                                  : make_uint4(0, 0, 0, 0);
+        }
+        __syncthreads();
     }
-    __syncthreads();
     if (DM == DM_COS) { // a2 of query `warp`
         float part = 0.f;
         for (uint32_t c = lane; c < nchunks; c += 32)
-            part = norm_add(part, query_norm_chunk<DM, SK>(sq[warp * nchunks + c]));
+            part = norm_add(part, query_norm_chunk<DM, SK>(qchunk(warp, c)));
         part = warp_sum(part);
         if (lane == 0)
             sa2[warp] = part;
@@ -119,7 +134,7 @@ __global__ void __launch_bounds__(kExWarps * 32) exact_block_kernel(const uint8_
                     const uint4 rv = __ldg(rp + c);
 #pragma unroll
                     for (int q = 0; q < kQT; ++q)
-                        accum_chunk<DM, SK>(acc[q], sq[q * nchunks + c], rv);
+                        accum_chunk<DM, SK>(acc[q], qchunk(q, c), rv);
                 }
             }
 #pragma unroll
@@ -280,6 +295,8 @@ void launch_merge_shards(const uint64_t* d_keys, const float* d_dists, size_t sh
     launch_merge_masked(d_keys, d_dists, shards, nq, k, d_out_keys, d_out_dists, nullptr, stream);
 }
 
+size_t device_smem_optin(); // engine.cu
+
 // exact_tc.cu
 bool exact_tc_applicable(int dist_mode, int scalar_kind, size_t n, size_t nq, size_t k, uint32_t row_bytes);
 bool exact_tc_defined(int dist_mode, int scalar_kind, size_t n, size_t k);
@@ -311,16 +328,33 @@ void launch_exact(int dist_mode, int scalar_kind, const uint8_t* d_data, size_t 
     float* part_dists = nullptr;
     LB_CUDA(cudaMallocAsync(&part_keys, blocks * nq * k * sizeof(uint64_t), stream));
     LB_CUDA(cudaMallocAsync(&part_dists, blocks * nq * k * sizeof(float), stream));
-    const size_t smem = (size_t)kQT * row_bytes + (size_t)kQT * kSub * 4 + (((size_t)kQT * k + 1) & ~(size_t)1) * 4 +
-                        (size_t)kQT * k * 8;
-    dim3 grid((unsigned)blocks, (unsigned)((nq + kQT - 1) / kQT));
+    // shared memory: the kQT staged query rows (unless they do not fit: QG), the sub-batch distances and the top-k lists
+    const size_t lists = (size_t)kQT * kSub * 4 + (((size_t)kQT * k + 1) & ~(size_t)1) * 4 + (size_t)kQT * k * 8;
+    const size_t optin = device_smem_optin();
+    const size_t static_smem = kQT * sizeof(float); // sa2
+    const bool qg = (size_t)kQT * row_bytes + lists + static_smem > optin;
+    const size_t smem = (qg ? 0 : (size_t)kQT * row_bytes) + lists;
+    if (smem + static_smem > optin) // k <= 1024 keeps the lists near 100 KB: never on sm_90
+        throw CudaError("exact search: the top-k lists do not fit in shared memory");
+    // grid.y is at most 65535: the query tiles go in slices of that many launches
+    const size_t tiles = (nq + kQT - 1) / kQT;
+    const size_t kMaxTiles = 65535;
     dispatch2(dist_mode, scalar_kind, [&](auto dm, auto sk) {
-        auto kern = exact_block_kernel<decltype(dm)::value, decltype(sk)::value>;
-        LB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, kExWarps * 32, smem, stream>>>(d_data, n, data_stride, d_queries, (uint32_t)nq, q_stride, row_bytes,
-                                                    (uint32_t)k, (uint32_t)rows_per_block, part_keys, part_dists, qmask);
-        LB_CUDA(cudaGetLastError());
-        count_launch();
+        auto launch = [&](auto kern) {
+            LB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            for (size_t t0 = 0; t0 < tiles; t0 += kMaxTiles) {
+                dim3 grid((unsigned)blocks, (unsigned)std::min(kMaxTiles, tiles - t0));
+                kern<<<grid, kExWarps * 32, smem, stream>>>(d_data, n, data_stride, d_queries, (uint32_t)nq, q_stride, row_bytes,
+                                                            (uint32_t)k, (uint32_t)rows_per_block, (uint32_t)t0, part_keys,
+                                                            part_dists, qmask);
+                LB_CUDA(cudaGetLastError());
+                count_launch();
+            }
+        };
+        if (qg)
+            launch(exact_block_kernel<decltype(dm)::value, decltype(sk)::value, true>);
+        else
+            launch(exact_block_kernel<decltype(dm)::value, decltype(sk)::value, false>);
     });
     launch_merge_masked(part_keys, part_dists, blocks, nq, k, d_keys, d_dists, qmask, stream);
     LB_CUDA(cudaFreeAsync(part_keys, stream));

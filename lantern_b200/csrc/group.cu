@@ -42,6 +42,8 @@
 
 namespace lb200 {
 
+size_t device_smem_optin(); // engine.cu: dynamic shared memory one CTA may opt in to
+
 namespace {
 
 constexpr int kGroupThreads = 128; // 4 independent warps per CTA (no CTA-wide synchronisation anywhere)
@@ -857,6 +859,10 @@ template <int DM, int SK, int NQ, bool PS = false> void group_launch_one(const G
 }
 template <int DM, int SK, int NQ, bool PS = false> int group_occupancy_one(size_t smem) {
     auto kern = group_search_kernel<DM, SK, NQ, PS>;
+    cudaFuncAttributes fa;
+    LB_CUDA(cudaFuncGetAttributes(&fa, kern));
+    if (smem + fa.sharedSizeBytes > device_smem_optin()) // deep rings of wide rows (LB200_GROUP_RING_SLOTS): refused by name
+        return 0;
     LB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int blocks = 0;
     LB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, kGroupThreads, smem));

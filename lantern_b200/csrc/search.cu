@@ -26,6 +26,8 @@
 
 namespace lb200 {
 
+size_t device_smem_optin(); // engine.cu: dynamic shared memory one CTA may opt in to
+
 namespace {
 
 template <class W> __device__ __forceinline__ void search_body(const SearchLaunch& p, const uint32_t R) {
@@ -203,6 +205,10 @@ template <class W> void launch_one(const SearchLaunch& p, uint32_t R, size_t sme
 
 template <class W> int occupancy_one(size_t smem, int threads) {
     auto kern = search_kernel_of<W>();
+    cudaFuncAttributes fa;
+    LB_CUDA(cudaFuncGetAttributes(&fa, kern));
+    if (smem + fa.sharedSizeBytes > device_smem_optin()) // a failed cudaFuncSetAttribute would also linger as the next call's last error
+        return 0;
     LB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int blocks = 0;
     LB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, threads, smem));

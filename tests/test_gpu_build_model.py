@@ -14,7 +14,7 @@ device add path with a strided tensor, and the full-bitmap clear of the walks' v
 import numpy as np
 import pytest
 
-from util import EXACT_FP32, describe_file_difference, exact_int_rows, hamming_rows
+from util import describe_file_difference, make_rows
 
 # name: (quant, metric, dims, rows, n, M, efc, build_batch, build_ratio, extra)
 #   rows: ("int", r) integers in [-r, r]; ("int0", r) the same plus all-zero and duplicate rows; ("i8", s) uniform in
@@ -38,38 +38,6 @@ CASES = {
     "b1-768-M32-b1024": ("b1", "hamming", 768, ("bits",), 8000, 32, 128, 1024, 4, ""),
     "b1-6144-M32-b64": ("b1", "hamming", 6144, ("bits",), 1500, 32, 64, 64, 16, ""),
 }
-
-
-def make_rows(port, quant, metric, dims, rows, n, seed):
-    """(input rows as passed to both builds, the same rows in the storage domain).  Asserts that every distance between two
-    of them is exact in fp32 (see the module docstring)."""
-    rng = np.random.default_rng(seed)
-    kind = rows[0]
-    if kind == "bits":
-        assert dims < EXACT_FP32
-        X = hamming_rows(n, dims, seed)
-        return X, X
-    if kind == "i8":
-        s = rows[1]
-        X = rng.uniform(-s, s, (n, dims)).astype(np.float32)
-        zero = rng.choice(n, n // 50, replace=False)  # |x| < 0.01: casts to an all-zero row (cos zero-norm rule)
-        X[zero] = rng.uniform(-0.0099, 0.0099, (len(zero), dims)).astype(np.float32)
-        r = min(100, int(np.floor(100 * s)))  # int8 cast: trunc(clamp(100 x, -100, 100))
-        assert (dims * (2 * r) ** 2 if metric == "l2sq" else dims * r * r) < EXACT_FP32
-        S = port.cast_f32(X, "i8")
-        assert np.abs(S.astype(np.int32)).max() <= r and (np.abs(S).sum(1) == 0).any()
-        return X, S
-    X = exact_int_rows(rng, n, dims, rows[1], metric)
-    if quant == "f16":
-        assert rows[1] <= 2048  # integers up to 2048 are f16 values: the cast is exact on both sides
-    if kind == "int0":  # zero-norm rows (both cos zero-norm cases) and exact duplicates (distance-0 ties)
-        X[rng.choice(n, n // 100, replace=False)] = 0
-        src, dst = rng.choice(n, (2, n // 50), replace=False)
-        X[dst] = X[src]
-    S = port.cast_f32(X, quant) if quant != "f32" else X
-    if quant == "f16":
-        assert np.array_equal(S.view(np.float16).astype(np.float32), X)
-    return X, S
 
 
 def batch_sizes(levels, batch_cap, build_ratio):
