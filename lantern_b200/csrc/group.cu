@@ -661,8 +661,9 @@ template <int DM, int SK, int NQ, bool PS = false> struct GroupWarp {
             if constexpr (PS) {
                 // a level-0 round that starts with a full top list: a candidate can enter only below td[L-1], and the radius
                 // only shrinks within the round, so screening against its start is safe (WalkerT::beam_impl's rule, which
-                // also skips a NaN radius)
-                const float radius = level == 0 && size == L ? top_d()[size - 1] : __int_as_float(0x7fffffff);
+                // also skips a NaN radius).  A greedy pass takes only a candidate strictly below cur_d: it is screened against
+                // cur_d (WalkerT::greedy's rule).
+                const float radius = level > 0 ? cur_d : level == 0 && size == L ? top_d()[size - 1] : __int_as_float(0x7fffffff);
                 if (radius == radius && n)
                     n = pscreen(n, radius);
                 cy_screen += (uint32_t)clock64() - cp1;

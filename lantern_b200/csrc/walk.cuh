@@ -792,7 +792,14 @@ template <class E> struct WalkerT : E {
                         sm.ctrl->n = n;
                 }
                 __syncthreads();
-                const uint32_t n = sm.ctrl->n;
+                const uint32_t n_all = sm.ctrl->n;
+                uint32_t n = n_all; // candidates measured
+                // Screened search walkers: a candidate with lb >= cur_d has d >= cur_d, which the strict '<' below never
+                // takes, and the screen keeps stored order, so the first minimum below cur_d is the same node.  cur_d is
+                // uniform across the CTA; a NaN cur_d (no candidate can be taken) skips the screen, as the beam's radius does.
+                if constexpr (E::kScreen)
+                    if (cur_d == cur_d)
+                        n = this->screen(n_all, cur_d);
                 eval(n);
                 __syncthreads();
                 // one pass of index.hpp:3304-3311: chain of strict improvements == first minimum below cur_d
@@ -803,7 +810,7 @@ template <class E> struct WalkerT : E {
                     if (d < best)
                         best = d, bi = (int)j;
                 }
-                st_dist += n, st_hops += 1;
+                st_dist += n_all, st_hops += 1; // the screen's rejects count as computed distances: the reference computes them
                 if (bi < 0)
                     break;
                 cur = sm.cand_id[bi], cur_d = best;

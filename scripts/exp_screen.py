@@ -10,8 +10,12 @@ the automatically chosen companion) and after each setting's first search (a for
 usage: python scripts/exp_screen.py [workload] ; env ROUNDS (default 3), STEPS (default 20), KNOBS (default 0,1,2; "auto" =
 unset), KERNELS (default "0": the "search_kernel" option, 0 = automatic, 1 = one CTA per query, 2 = one warp per query;
 "1w2" = one CTA of 2 warps per query with 12 KB rings, LB200_SEARCH_WARPS=2 LB200_RING_BYTES=12288), DATA (structured |
-gauss), OUT (directory for the JSON)"""
-import json, os, sys, time
+gauss), OUT (directory for the JSON), INDEX (an index file: loaded instead of building the graph when it exists, else written
+after the build, so that two builds of the engine can be timed on one graph in alternating processes).
+Per setting it also prints upper_hops_per_query and screened_per_query.  Every candidate of a greedy pass goes through the
+screen (unless the walk's distance is NaN), so on one graph screened_per_query minus that of a build whose descent is not
+screened is the descent's candidates per query, and that over upper_hops_per_query the mean fill of the lists it visits."""
+import hashlib, json, os, sys, time
 sys.path.insert(0, '.')
 import numpy as np, torch
 import bench
@@ -28,17 +32,26 @@ n, dim, B, k, ef = wl["n"], wl["dim"], wl["batch"], wl["k"], wl["ef"]
 dev = torch.device("cuda", 0)
 free0, total = torch.cuda.mem_get_info()
 pool = 4
+index_file = os.environ.get("INDEX")
+load = bool(index_file) and os.path.exists(index_file)
 if data == "gauss":
-    X = torch.randn((n, dim), generator=torch.Generator(device=dev).manual_seed(bench.SEED_CORPUS), device=dev)
+    if not load:
+        X = torch.randn((n, dim), generator=torch.Generator(device=dev).manual_seed(bench.SEED_CORPUS), device=dev)
     Q = torch.randn((pool * B, dim), generator=torch.Generator(device=dev).manual_seed(bench.SEED_QUERY), device=dev)
 else:
-    X = bench.structured_torch(n, dim, bench.SEED_CORPUS, dev)
+    if not load:
+        X = bench.structured_torch(n, dim, bench.SEED_CORPUS, dev)
     Q = bench.structured_torch(pool * B, dim, bench.SEED_QUERY, dev)
 idx = api.Index(dim, wl["metric"], "f32", M=wl["M"], efc=wl["efc"], ef=ef)
-idx.reserve(n)
 t = time.time()
-idx.add_batch_device(np.arange(1, n + 1, dtype=np.uint64), X.data_ptr(), n, dim * 4, "f32")
-idx.build()
+if load:
+    idx.load(index_file)  # load_buffer chooses the same basis bits from the same rows
+else:
+    idx.reserve(n)
+    idx.add_batch_device(np.arange(1, n + 1, dtype=np.uint64), X.data_ptr(), n, dim * 4, "f32")
+    idx.build()
+    if index_file:
+        idx.save(index_file)
 torch.cuda.synchronize()
 mem = {"total_gb": total / 1e9, "used_before_gb": (total - free0) / 1e9}
 mem["used_after_build_gb"] = (total - torch.cuda.mem_get_info()[0]) / 1e9
@@ -83,7 +96,7 @@ for kern, knob in [("0", "auto")] + settings:  # outputs and counters of every p
         st = idx.last_stats()
         outs.append((ok.cpu().numpy().copy(), od.cpu().numpy().view(np.uint32).copy(), oc.cpu().numpy().copy(),
                      st["computed_distances"], st["base_pops"], st["upper_hops"], st["full_rows_read"], st["screen_kind"],
-                     st["screen_dims"], st["search_kernel"]))
+                     st["screen_dims"], st["search_kernel"], st["algorithmic_bytes"]))
         cy += [st[c] for c in CYCLES]
     ref[name(kern, knob)], cyc[name(kern, knob)] = outs, cy
     print("%s: %d checked batches in %.2f s, kind %d, %d codes per candidate, kernel %d" % (
@@ -114,15 +127,24 @@ for r in range(rounds):
 auto = name("0", "auto")
 out = {"workload": wl_name, "data": data, "identical_outputs_and_counters": bool(same), "memory": mem,
        "gpu": torch.cuda.get_device_name(0), "auto_screen_kind": ref[auto][0][7], "auto_screen_dims": ref[auto][0][8],
-       "auto_search_kernel": ref[auto][0][9]}
+       "auto_search_kernel": ref[auto][0][9],
+       # keys, distance bits and counts of the checked batches: equal across processes = the same outputs
+       "outputs_sha256": hashlib.sha256(b"".join(a.tobytes() for o in ref[names[0]] for a in o[:3])).hexdigest()}
 for nm in names:
     v = np.array(res[nm])
     cd = sum(o[3] for o in ref[nm])
     fr = sum(o[6] for o in ref[nm])
     cy = cyc[nm]
+    # candidates that went through the screen, from the byte count: the inverse of Index::last_stats()'s algorithmic_bytes
+    # (engine.cu, DESIGN.md 4.1), which assumes f32 rows of 4 * dim bytes, M0 = 2M, one query row per query and a record of
+    # 64 bytes for k <= 48, else 128 (projected) or a code row + 16 bytes of metadata (int8): change it with that formula
+    kind, sd = ref[nm][0][7], ref[nm][0][8]
+    rest = sum(o[10] - o[6] * dim * 4 - o[4] * (4 + 8 * wl["M"]) - o[5] * (4 + 4 * wl["M"]) - B * dim * 4 for o in ref[nm])
+    screened = rest / ({1: dim + 16, 2: 64 if sd <= 48 else 128}[kind]) if kind else 0
     out[nm] = {"qps_median": float(np.median(v)), "qps_min": float(v.min()), "qps_max": float(v.max()),
                "kernel_ms_median": float(np.median(kern_ms[nm])), "dist_evals_per_query": cd / (pool * B),
                "full_rows_read_per_query": fr / (pool * B), "full_rows_frac": fr / cd,
+               "upper_hops_per_query": sum(o[5] for o in ref[nm]) / (pool * B), "screened_per_query": screened / (pool * B),
                "screen_kind": ref[nm][0][7], "codes_per_candidate": ref[nm][0][8], "search_kernel": ref[nm][0][9],
                "cycle_split": {c[len("owner_cycles_"):]: (float(x / cy.sum()) if cy.sum() else 0.0) for c, x in zip(CYCLES, cy)}}
 for nm in names[1:]:
